@@ -1,6 +1,6 @@
-"""bench.py — headline benchmark of the MichiGAN hot path on B200.
+"""bench.py — headline benchmark of the MichiGAN hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload both|gen_fwd|train_step]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload both|gen_fwd|train_step] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -12,14 +12,17 @@ BASELINE.json's metric has two halves, both measured by the default run and prin
   train_step  configs[2]: the full G+D train iteration (hinge GAN + GAN-feature losses, Adam TTUR), batch 8 per GPU,
               512x512 synthetic; same keys as the top level (value, ms_per_step, e2e, roofline, gpu_launches).
 
-  value       images/s, whole job, inputs already resident in HBM, CUDA-event timed, max over ranks.  A timed BLOCK is
-              exactly --steps steps between barrier + synchronize pairs; blocks are repeated until the leg has run for
-              >= 2 s (at most 8 blocks) and the MEDIAN block is reported (all block times are listed in `blocks_ms`).
+  value       images/s, whole job, inputs already resident in HBM, CUDA-event timed, max over ranks.  The timed BLOCK is
+              exactly --steps steps between barrier + synchronize pairs (its time is listed in `blocks_ms`).
   e2e         images/s through the public API with pinned HOST buffers: H2D of the data dict and D2H of the result
               (image / loss scalars) inside the timed region
   roofline    the dominant kernel timed alone, live; roofline_worst: the kernel furthest below its roofline
   cpu_baseline / --impl reference   the reference's own CPU implementation on the host cores: the UNMODIFIED reference
               code staged under baseline/_ref (kind "reference") when present, else the CPU oracle port (kind "port")
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float32): gen_fwd_image
+(the generated images), train_step_generated and train_step_losses.  Inputs and weights are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -38,9 +41,8 @@ BATCH_PER_GPU = 8
 SIZE = 512
 G_FWD_GFLOP_PER_IMG = 1114.2  # SURVEY.md §8d / BASELINE.md §3 (2*MAC, convs only)
 TRAIN_GFLOP_PER_IMG = 4775.8  # SURVEY.md §8d: G step + D step, hinge GAN + GAN-feature losses
-MIN_LEG_SECONDS = 2.0
-MAX_BLOCKS = 8
-CPU_THREADS = 32              # fixed: PyTorch's CPU convs stop scaling (and regress) beyond ~32 threads on the B200 hosts
+CPU_THREADS = 32              # fixed: PyTorch's CPU convs stop scaling (and regress) beyond ~32 threads
+DUMP_BYTES_MAX = 64 << 20
 
 
 def parse():
@@ -54,6 +56,8 @@ def parse():
                          "per-GPU work: the train step with --use_ig (frozen orientation-inpainting net, run twice per iteration)")
     ap.add_argument("--batch", type=int, default=BATCH_PER_GPU)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all)")
     return ap.parse_args()
 
 
@@ -63,11 +67,12 @@ def peaks():
         with open(path) as f:
             p = json.load(f)
         return p, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "data-sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason samples during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle-reason samples during the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -223,12 +228,6 @@ def run_reference_arm(a):
 
 
 # ================================================================================================ single-kernel rooflines
-# DRAM traffic of one launch of the dominant kernel from the `ncu --set full` capture committed under profiles/
-# (dram__bytes_read.sum + dram__bytes_write.sum at N=8); algorithmic bytes at N=8 (2,097,152 pixels): actv fp16 128 ch 537 MB +
-# x fp32 128 ch at half resolution 268 MB + weights 0.6 MB read, bf16 hi+lo 128 ch 1074 MB written - the kernel moves its
-# algorithmic bytes and nothing more.
-NCU_TRAFFIC_BYTES_N8 = 809.607936e6 + 1027.305e6
-NCU_TRAFFIC_SOURCE = "profiles/r02_ncu_spade_gemm_f16_tma.txt"
 
 
 def _time_kernel(f, reps=5):
@@ -237,7 +236,7 @@ def _time_kernel(f, reps=5):
         f()
     times = []
     for _ in range(reps):
-        flush.zero_()  # evict L2 (126 MB) between timed launches
+        flush.zero_()  # evict L2 (50 MB) between timed launches
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         f()
@@ -261,12 +260,12 @@ def dominant_kernel_roofline(batch):
     v = torch.ones(128, device=dev)
     if precision.mode() == "tf32":
         wp = ops.pack_weight_gb(wg, wg)
-        kind = "kind::tf32"
+        kind = "tf32 operands"
         f = lambda: ops.conv_igemm(actv, wp, 128, 3, 3, 1, 1, act=2, round_out=True, spade=(xs, 1, v, v, v, v))
     else:
         a16 = actv.half()
         wp = ops.pack_weight_gb16(wg, wg)
-        kind = "kind::f16"
+        kind = "fp16 operands"
         f = lambda: ops.conv_igemm(a16, wp, 128, 3, 3, 1, 1, act=2, a_fmt=ops.F16, spade=(xs, 1, v, v, v, v),
                                    out16=(ops.BF16, True), want_f32=False)
     ms = _time_kernel(f)
@@ -286,13 +285,13 @@ def worst_kernel_roofline(batch):
     if precision.mode() == "tf32":
         wp = ops.pack_weight(w, None, True)
         f = lambda: ops.conv_igemm(x, wp, 64, 3, 3, 1, 1, bias=b)
-        kind = "kind::tf32, one pass"
+        kind = "tf32 operands, one pass"
     else:
         hi = x.bfloat16()
         lo = (x - hi.float()).bfloat16()
         wp = ops.pack_weight16(w, None, ops.BF16, split=True)
         f = lambda: ops.conv_igemm(hi, wp, 64, 3, 3, 1, 1, bias=b, a_fmt=ops.BF16, x_lo=lo)
-        kind = "kind::f16 bf16 hi+lo split"
+        kind = "bf16 hi+lo split operands"
     ms = _time_kernel(f)
     flops = 2.0 * batch * SIZE * SIZE * 1152 * 64
     return flops / (ms * 1e-3) / 1e12, ms, flops, kind
@@ -310,10 +309,10 @@ def wgrad_kernel_roofline(batch):
         dy16, x16 = dy.bfloat16(), x.bfloat16()
         del dy, x
         f = lambda: ops.conv_wgrad16(dy16, x16, 3, 3, 1, 1)
-        kind = "kind::f16 (bf16 operands)"
+        kind = "bf16 operands"
     else:
         f = lambda: ops.conv_wgrad(dy, x, 3, 3, 1, 1)
-        kind = "kind::tf32"
+        kind = "tf32 operands"
     ms = _time_kernel(f, reps=3)
     flops = 2.0 * batch * SIZE * SIZE * 1152 * 256
     return flops / (ms * 1e-3) / 1e12, ms, flops, kind
@@ -321,8 +320,8 @@ def wgrad_kernel_roofline(batch):
 
 # ================================================================================================ native arm
 def timed_blocks(step, steps, world):
-    """Repeat [barrier+sync | e0 | `steps` x step | e1 | barrier+sync] until >= MIN_LEG_SECONDS have been timed; every block
-    time is the max over ranks (so all ranks agree on when to stop).  Returns the list of block times in ms."""
+    """[barrier+sync | e0 | `steps` x step | e1 | barrier+sync]: exactly `steps` timed steps; the block time is the max over
+    ranks.  Returns the list of block times in ms (one block)."""
     import torch.distributed as dist
 
     def barrier():
@@ -332,22 +331,20 @@ def timed_blocks(step, steps, world):
 
     blocks = []
     timed_blocks.host_ms = []          # CPU time to ISSUE each block (no synchronisation inside a block)
-    while True:
-        barrier()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        t0 = time.perf_counter()
-        for _ in range(steps):
-            step()
-        timed_blocks.host_ms.append((time.perf_counter() - t0) * 1e3)
-        e1.record()
-        barrier()
-        ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
-        if world > 1:
-            dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-        blocks.append(float(ms.item()))
-        if sum(blocks) >= MIN_LEG_SECONDS * 1e3 or len(blocks) >= MAX_BLOCKS:
-            return blocks
+    barrier()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    t0 = time.perf_counter()
+    for _ in range(steps):
+        step()
+    timed_blocks.host_ms.append((time.perf_counter() - t0) * 1e3)
+    e1.record()
+    barrier()
+    ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
+    if world > 1:
+        dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+    blocks.append(float(ms.item()))
+    return blocks
 
 
 def median(v):
@@ -378,7 +375,7 @@ def gen_fwd_leg(a, rank, world, local, model):
         torch.cuda.synchronize()
 
         def step():
-            return model.generate_fake(pre[0], pre[2], pre[4], pre[1], pre[3], pre[5])
+            model.last_outputs = {"gen_fwd_image": model.generate_fake(pre[0], pre[2], pre[4], pre[1], pre[3], pre[5])}
 
         for _ in range(a.warmup):
             step()
@@ -429,7 +426,7 @@ def gen_fwd_leg(a, rank, world, local, model):
             main_stream.synchronize()
 
         e2e_run(max(2, a.warmup // 2 + 1))
-        e2e_steps = a.steps * max(1, min(MAX_BLOCKS, len(blocks)))
+        e2e_steps = a.steps
         barrier()
         t0 = time.perf_counter()
         e2e_run(e2e_steps)
@@ -449,9 +446,9 @@ def gen_fwd_leg(a, rank, world, local, model):
         "config": {"workload": "generator-only forward (netG=spadeb ngf64, 109.5M params, train-mode statistics, no grad), "
                                "batch %d/GPU, 512x512 synthetic mask/orient/ref inputs" % batch,
                    "global_batch": batch * world, "parallelism": "dp%d" % world,
-                   "l2": "no explicit flush: each step streams multi-GB NHWC activations (>> 126 MB L2)",
+                   "l2": "no explicit flush: each step streams multi-GB NHWC activations (>> 50 MB L2)",
                    "algorithmic_gflop_per_image": G_FWD_GFLOP_PER_IMG,
-                   "timing": "median of %d blocks of %d steps (>= %.0f s timed)" % (len(blocks), a.steps, MIN_LEG_SECONDS)},
+                   "timing": "%d timed steps" % a.steps},
         "blocks_ms": blocks,
         "achieved_tflops_step": G_FWD_GFLOP_PER_IMG * batch / ms_step,
         "e2e": {"value": world * batch * e2e_steps / t_e2e, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -483,8 +480,9 @@ def train_step_leg(a, rank, world, local, model, use_ig=False):
         torch.cuda.synchronize()
 
     def step():
-        g, d, _ = train_iteration(wrap, optG, optD, dict(dev))
+        g, d, generated = train_iteration(wrap, optG, optD, dict(dev))
         last["losses"] = {**g, **d}
+        last["generated"] = generated
 
     for _ in range(a.warmup):
         step()
@@ -498,6 +496,8 @@ def train_step_leg(a, rank, world, local, model, use_ig=False):
     launches = (_lib.launch_count() - l0) // len(blocks)
     clocks = sampler.stop() if rank == 0 else None
     ms_block = median(blocks)
+    model.last_outputs = {"train_step_generated": last["generated"].detach(),
+                          "train_step_losses": torch.stack([v.detach().float().mean() for v in last["losses"].values()])}
 
     # ---- end to end: every step's inputs come from pinned HOST tensors (copied on a second stream into one of two device
     # buffers while the previous step computes - a prefetching loader) and every step ends with its loss scalars read back to the
@@ -558,7 +558,7 @@ def train_step_leg(a, rank, world, local, model, use_ig=False):
                    "l2": "no explicit flush: multi-GB activations per step",
                    "algorithmic_gflop_per_image": TRAIN_GFLOP_PER_IMG + (2 * 151.9 if use_ig else 0.0),
                    "use_ig": bool(use_ig),
-                   "timing": "median of %d blocks of %d steps" % (len(blocks), a.steps),
+                   "timing": "%d timed steps" % a.steps,
                    "syncbn_exchange": exchange_backend(), "grad_allreduce": "in-backward staged NCCL all-reduce (AVG) of a flat fp32 buffer"},
         "blocks_ms": blocks,
         "achieved_tflops_step": (TRAIN_GFLOP_PER_IMG + (2 * 151.9 if use_ig else 0.0)) * batch / ms_step,
@@ -584,6 +584,8 @@ def run_native(a):
     from michigan_b200.pix2pix_model import Pix2PixModel
     from michigan_b200.synth import fill_state_dict
 
+    import random
+    random.seed(0)
     torch.manual_seed(0)
     use_ig = a.workload == "train_step_ig"
     extra = {}
@@ -604,27 +606,29 @@ def run_native(a):
     model.train()
 
     line = None
+    dumps = {}
     if a.workload in ("both", "gen_fwd"):
         line = gen_fwd_leg(a, rank, world, local, model)
+        dumps.update(model.last_outputs)
     train = None
     if a.workload in ("both", "train_step", "train_step_ig"):
         train = train_step_leg(a, rank, world, local, model, use_ig)
+        dumps.update(model.last_outputs)
+    if rank == 0 and a.dump_outputs:
+        dump_outputs(a.dump_outputs, dumps)
     if rank == 0:
         pk, pk_kind = peaks()
         peak_tf = float(pk["bf16_tflops"])
         if line is not None:
             tf, kms, kflops, kkind = dominant_kernel_roofline(a.batch)
             line["roofline"] = {
-                "kernel": "igemm_tf32_kernel<1,16> (fused SPADE gamma|beta implicit GEMM + modulate + LeakyReLU, up_3.norm_0 shape, tcgen05 %s)" % kkind,
-                "bound": "tensor", "achieved": tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": tf / peak_tf,
-                "traffic": NCU_TRAFFIC_BYTES_N8 * a.batch / 8 if kkind == "kind::f16" else None,
-                "traffic_unit": "bytes per launch (dram read + write, ncu --set full, %s)" % NCU_TRAFFIC_SOURCE,
-                "peak_kind": "%s bf16 dense burst (MEASURED_PEAKS.json)%s" % (
-                    pk_kind, "; kind::tf32 issues at half the bf16 rate" if kkind == "kind::tf32" else ""),
+                "kernel": "conv3x3_group_kernel<1,16> (fused SPADE gamma|beta implicit GEMM + modulate + LeakyReLU, up_3.norm_0 shape, wgmma %s)" % kkind,
+                "bound": "tensor", "achieved": tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": tf / peak_tf, "traffic": None,
+                "peak_kind": "%s bf16 dense%s" % (pk_kind, "; tf32 runs at half the bf16 rate" if kkind == "tf32 operands" else ""),
                 "ms_per_launch": kms, "flops_per_launch": kflops}
             wtf, wms, wflops, wkind = worst_kernel_roofline(a.batch)
             line["roofline_worst"] = {
-                "kernel": "conv3x3_group_kernel<0,16> (3x3 implicit-GEMM conv on the halo-patch + M-tile-group schedule, up_3.conv_0 shape 128->64 at 512x512, %s)" % wkind,
+                "kernel": "conv3x3_group_kernel<0,16> (3x3 implicit-GEMM conv on the halo-patch + M-tile-group schedule, up_3.conv_0 shape 128->64 at 512x512, wgmma %s)" % wkind,
                 "bound": "tensor", "achieved": wtf, "peak": peak_tf, "unit": "TFLOP/s", "frac": wtf / peak_tf, "traffic": None,
                 "note": "algorithmic FLOPs (one product per MAC); the split-precision form issues 3 products per MAC",
                 "ms_per_launch": wms, "flops_per_launch": wflops}
@@ -632,9 +636,9 @@ def run_native(a):
             gtf, gms, gflops, gkind = wgrad_kernel_roofline(a.batch)
             train["roofline"] = {
                 "kernel": "wgrad_tf32_kernel (weight-gradient GEMM, SPADE gamma|beta wgrad of up_3: K = N*512*512 pixels, 256 x 1152 outputs, "
-                          "MN-major operands, tcgen05 %s)" % gkind,
+                          "MN-major operands, mma.sync %s)" % gkind,
                 "bound": "tensor", "achieved": gtf, "peak": peak_tf, "unit": "TFLOP/s", "frac": gtf / peak_tf, "traffic": None,
-                "peak_kind": "%s bf16 dense burst (MEASURED_PEAKS.json)" % pk_kind,
+                "peak_kind": "%s bf16 dense" % pk_kind,
                 "ms_per_launch": gms, "flops_per_launch": gflops}
         if line is None:
             line = train
@@ -648,6 +652,21 @@ def run_native(a):
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(dirname, arrays):
+    """Each tensor -> dirname/<name>.npy as float32.  When the whole set would pass DUMP_BYTES_MAX, every tensor larger than its
+    share is replaced by a fixed (seed 0) sample of its flattened elements, in index order."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    total = sum(t.numel() * 4 for t in arrays.values())
+    share = DUMP_BYTES_MAX // max(1, len(arrays))
+    for name, t in arrays.items():
+        v = t.detach().float().cpu().numpy()
+        if total > DUMP_BYTES_MAX and v.size * 4 > share:
+            idx = np.sort(np.random.default_rng(0).choice(v.size, share // 4, replace=False))
+            v = v.reshape(-1)[idx]
+        np.save(os.path.join(dirname, name + ".npy"), np.ascontiguousarray(v, dtype=np.float32))
 
 
 DTYPE_NOTE = {

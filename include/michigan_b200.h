@@ -1,4 +1,4 @@
-/* michigan_b200 — C ABI of libmichigan_sm100.so (hand-written CUDA for sm_100a).
+/* michigan_b200 — C ABI of libmichigan_sm90.so (hand-written CUDA for sm_90a).
  *
  * This is the drop-in boundary for the MichiGAN data-parallel hot path.  The reference has no
  * native code: every entry point below replaces a group of PyTorch ops that the reference calls
@@ -48,7 +48,7 @@ int mg_debug_igemm_prof(unsigned long long* host16);
 #define MG_EPI_BIAS 0  /* y = act((acc*pscale + bias + residual) ...) (+ blend)            */
 #define MG_EPI_SPADE 1 /* y = act(xhat*(1+gamma)+beta), gamma|beta = the two halves of acc */
 
-/* Implicit-GEMM convolution on tcgen05 tensor cores (TF32 operands, fp32 accumulate in TMEM).
+/* Implicit-GEMM convolution on wgmma tensor cores (TF32 / fp16 / bf16 operands, fp32 accumulate).
  * Replaces nn.Conv2d / F.conv2d at: normalization.py:97-98,112-113 (mlp_gamma/mlp_beta, fused with
  * the modulation of normalization.py:116 and the LeakyReLU of architecture.py:84-85),
  * architecture.py:31-34,70-71,79 (conv_0/conv_1/conv_s), MaskGAN_networks.py:162-168 (ConvBlock
@@ -235,7 +235,7 @@ typedef struct mg_sn_desc {
 int mg_spectral_norm_batched(const void* descs, int n_layers, int max_O, int max_K, int training, float eps,
                              void* stream);
 
-/* Weight gradient of the implicit-GEMM convs on tcgen05 (TF32, MN-major operands, split-K over
+/* Weight gradient of the implicit-GEMM convs on tensor cores (TF32, MN-major operands, split-K over
  * pixels): dw[co][(kh*KW+kw)*Cin+ci] = sum_pix dy[pix,co] * x[pix*stride - pad + (kh,kw), ci].
  * dy [N,OH,OW,Cout], x [N,H,W,Cin] NHWC; dw has the packed layout of mg_pack_weight (autograd of
  * nn.Conv2d at the call sites listed for mg_conv_igemm). */

@@ -1,4 +1,4 @@
-"""ctypes binding of libmichigan_sm100.so (C ABI declared in include/michigan_b200.h).
+"""ctypes binding of libmichigan_sm90.so (C ABI declared in include/michigan_b200.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, an exception is
 raised.  The product path never routes through PyTorch eager or the CPU oracle.
@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # MICHIGAN_B200_LIB: tools/ select the -DMG_PROBES build (timing experiments); the product always loads the in-tree release library
-LIB_PATH = os.environ.get("MICHIGAN_B200_LIB") or os.path.join(_HERE, "lib", "libmichigan_sm100.so")
+LIB_PATH = os.environ.get("MICHIGAN_B200_LIB") or os.path.join(_HERE, "lib", "libmichigan_sm90.so")
 
 c_f32p = C.c_void_p  # device pointers travel as integers (tensor.data_ptr())
 
@@ -141,7 +141,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise MichiganNativeError(
-            "libmichigan_sm100.so not found at %s - run `python -m michigan_b200.build` "
+            "libmichigan_sm90.so not found at %s - run `python -m michigan_b200.build` "
             "(the CUDA extension is mandatory; there is no fallback path)" % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, argtypes in SIGNATURES.items():
@@ -158,7 +158,7 @@ def load():
 def check(rc, what=""):
     if rc != 0:
         msg = load().mg_last_error().decode("utf-8", "replace")
-        raise MichiganNativeError("%s failed (status %d): %s" % (what or "libmichigan_sm100 call", rc, msg))
+        raise MichiganNativeError("%s failed (status %d): %s" % (what or "libmichigan_sm90 call", rc, msg))
 
 
 def set_tuning(name, value):

@@ -1,4 +1,4 @@
-"""Build libmichigan_sm100.so (hand-written CUDA, sm_100a only) in-tree with nvcc.
+"""Build libmichigan_sm90.so (hand-written CUDA, sm_90a only) in-tree with nvcc.
 
     python -m michigan_b200.build [--force]
 
@@ -12,11 +12,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
-LIB_PATH = os.path.join(LIB_DIR, "libmichigan_sm100.so")
+LIB_PATH = os.path.join(LIB_DIR, "libmichigan_sm90.so")
 SOURCES = ["mg_api.cu", "mg_igemm.cu", "mg_aux.cu", "mg_wgrad.cu", "mg_bwd.cu", "mg_segconv.cu", "mg_peer.cu", "mg_loss.cu", "mg_conv3x3.cu", "mg_synth.cu", "mg_orient.cu", "mg_attn.cu"]  # missing files are skipped
 HEADERS = ["mg_ptx.cuh", "mg_internal.h", "mg_epilogue.cuh", os.path.join("..", "..", "include", "michigan_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math=false",
 ]
 
@@ -38,8 +38,8 @@ def _stale():
 
 
 def build(force=False, verbose=False, probes=False):
-    """Compile every CUDA source for sm_100a and link the shared library. Returns its path.
-    probes=True builds the tools-only variant libmichigan_sm100_probes.so (-DMG_PROBES: what-if switches that skip work
+    """Compile every CUDA source for sm_90a and link the shared library. Returns its path.
+    probes=True builds the tools-only variant libmichigan_sm90_probes.so (-DMG_PROBES: what-if switches that skip work
     and the clock64() role profiles; never loaded by the product, select it with MICHIGAN_B200_LIB=<path>)."""
     lib_path = LIB_PATH.replace(".so", "_probes.so") if probes else LIB_PATH
     if not force and not probes and not _stale():

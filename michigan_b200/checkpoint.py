@@ -1,5 +1,5 @@
 """Checkpoint I/O with the reference's file layout (util/util.py:195-231: `<checkpoints_dir>/<name>/<epoch>_net_<label>.pth`
-= a CPU state dict with the network's own keys), B200-side behaviour:
+= a CPU state dict with the network's own keys), device-side behaviour:
 
   * the reference's `save_network` moves the WHOLE network to the CPU and back in the middle of training
     (`net.cpu().state_dict()`; `net.cuda()`), on every DataParallel thread's shared module; here the parameters stay

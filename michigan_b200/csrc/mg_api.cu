@@ -115,6 +115,63 @@ int encode_tensor_map(CUtensorMap* map, void* gaddr, CUtensorMapDataType dtype, 
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------- order-independent sums
+// The buffers come from a memory pool of this library (one per device, created on first use) that keeps freed blocks
+// cached: the train step allocates a few MB per backward kernel, and a pool that trimmed at every synchronisation would
+// hand them back to the driver each step.  Allocation stays stream-ordered, so concurrent streams never share a buffer.
+static cudaMemPool_t acc64_pool(int dev) {
+    static std::mutex mu;
+    static cudaMemPool_t pools[64] = {};
+    std::lock_guard<std::mutex> lock(mu);
+    if (dev < 0 || dev >= 64) return nullptr;
+    if (!pools[dev]) {
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = dev;
+        cudaMemPool_t pool = nullptr;
+        if (cudaMemPoolCreate(&pool, &props) != cudaSuccess) return nullptr;
+        unsigned long long keep = ~0ull;
+        cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+        pools[dev] = pool;
+    }
+    return pools[dev];
+}
+
+int acc64_alloc(double** acc, size_t n, cudaStream_t stream) {
+    *acc = nullptr;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaMemPool_t pool = acc64_pool(dev);
+    if (!pool) return set_error(-1, "acc64_alloc: no memory pool for device %d", dev);
+    cudaError_t e = cudaMallocFromPoolAsync(reinterpret_cast<void**>(acc), n * sizeof(double), pool, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(*acc, 0, n * sizeof(double), stream);
+    if (e != cudaSuccess) return set_error((int)e, "acc64_alloc: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+__global__ void acc64_fold_kernel(const double* __restrict__ acc, float* __restrict__ dst, long long n, int add) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        dst[i] = (add ? dst[i] : 0.f) + (float)acc[i];
+}
+
+int acc64_fold(const double* acc, float* dst, size_t n, int add, cudaStream_t stream) {
+    long long blocks = ((long long)n + 255) / 256;
+    if (blocks > 4096) blocks = 4096;
+    if (blocks < 1) blocks = 1;
+    acc64_fold_kernel<<<(int)blocks, 256, 0, stream>>>(acc, dst, (long long)n, add);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error((int)e, "acc64_fold: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+int acc64_free(double* acc, cudaStream_t stream) {
+    cudaError_t e = cudaFreeAsync(acc, stream);
+    if (e != cudaSuccess) return set_error((int)e, "acc64_free: %s", cudaGetErrorString(e));
+    return 0;
+}
+
 }  // namespace mg
 
 extern "C" int mg_version(void) { return MG_ABI_VERSION; }

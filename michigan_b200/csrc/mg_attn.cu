@@ -1,7 +1,7 @@
-// michigan_b200 — row softmax that emits tensor-core operands (sm_100a).
+// michigan_b200 — row softmax that emits tensor-core operands (sm_90a).
 //
 // InpaintGenerator's SelfAttention (reference models/networks/generator.py:467-485) is softmax(Q K^T) V over the 4096
-// tokens of a 64x64 map.  Both products run on the tcgen05 implicit-GEMM kernel as 1x1 "convolutions" whose weight operand
+// tokens of a 64x64 map.  Both products run on the wgmma implicit-GEMM kernel as 1x1 "convolutions" whose weight operand
 // is the per-image K (resp. V^T) matrix; this kernel is the piece in between: numerically stable softmax of every score row,
 // written directly in the operand format of the second product (fp32 rounded to TF32, or 16-bit hi / hi+lo), so the
 // probabilities are never re-read for a conversion pass.

@@ -1,4 +1,4 @@
-// michigan_b200 — CUDA-core kernels around the tcgen05 implicit GEMM: weight packing, thin
+// michigan_b200 — CUDA-core kernels around the tensor-core implicit GEMM: weight packing, thin
 // (3/4/7-channel) direct convolutions, normalisation statistics, input preparation, pooling.
 // These are the HBM-bound pieces of the path: coalesced 128-bit accesses, NHWC, no tensor cores.
 #include <cuda_runtime.h>
@@ -966,7 +966,7 @@ extern "C" int mg_conv_thin(const mg_thin_args* a, void* stream) {
         thin_conv_kernel<CI, CP><<<grid, 256, smem, ST(stream)>>>(*a, tiles_w, tiles_h, num_tiles);          \
     } while (0)
     const int use_gemm = tune(TK_THIN_GEMM);
-    // measured on B200: the register-tiled variant wins for Cout = 64 (k7 / k4 layers), the lane-per-channel one for Cout = 128
+    // the register-tiled variant serves Cout = 64 (k7 / k4 layers), the lane-per-channel one Cout = 128
     if ((use_gemm == 2 && a->Cout == 128) || (use_gemm >= 1 && a->Cout == 64)) {
 #define LAUNCH_TG(CI, CT)                                                                                     \
     do {                                                                                                      \
@@ -1307,7 +1307,7 @@ extern "C" int mg_pack_weight_gb16(const float* wg, const float* wb, void* out, 
 
 // ------------------------------------------------------------------------------------ channel padding to 32
 // out[n,i,j,0:32] = (c < CinP ? in[n, src_i, src_j, c] : 0) with optional nearest down-sampling by R (segmap) and
-// reflection padding by p (out is then [N,H+2p,W+2p,32]); values TF32-rounded: operand of the tcgen05 weight-gradient
+// reflection padding by p (out is then [N,H+2p,W+2p,32]); values TF32-rounded: operand of the tensor-core weight-gradient
 // kernel for the thin (3/4/7-channel input) convolutions.
 namespace mg {
 __global__ void pad_channels32_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int H, int W, int CinP, int R,

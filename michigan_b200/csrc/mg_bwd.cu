@@ -293,7 +293,7 @@ __global__ void in_bwd_apply_kernel(const float* __restrict__ df, const float* _
 // weight gradient of a thin conv: dwt[tap][ci][co] += sum_pix x[pix*s - pad + tap][ci] * dz[pix][co]
 // block: 8 output rows x 16 cols tile (same tiling as the forward), thread (co, part) accumulates a slice of taps.
 __global__ void __launch_bounds__(256)
-thin_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dz, float* __restrict__ dwt, int N, int H, int W,
+thin_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dz, double* __restrict__ dwt, int N, int H, int W,
                   int CinP, int OH, int OW, int Cout, int KH, int KW, int s, int pad, int pad_mode, int R, int tiles_w,
                   int tiles_h, int num_tiles) {
     extern __shared__ __align__(16) float sm[];
@@ -351,16 +351,16 @@ thin_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dz, flo
         }
     }
     if (part < parts)
-        for (int k = k0; k < k1; ++k) atomicAdd(dwt + (size_t)k * Cout + co, acc[k - k0]);
+        for (int k = k0; k < k1; ++k) atomicAdd(dwt + (size_t)k * Cout + co, (double)acc[k - k0]);
 }
 
-// Register-tiled weight gradient of a thin conv (replaces the tensor-core route for Cin <= 8: with N = 32 padded channels
-// every tcgen05.mma sits on its ~100-cycle issue floor, profiles/r01_mma_rate_microbench.log).  Thread = (group of 4 output
+// Register-tiled weight gradient of a thin conv (replaces the tensor-core route for Cin <= 8, which pads N to 32 channels).  Thread = (group of 4 output
 // channels) x (KPT of the KH*KW*CinP weight columns): per pixel one float4 of dz and KPT input values from shared memory
-// feed 4*KPT FMAs; the per-CTA partial sums stay in registers across all its tiles and are added atomically at the end.
+// feed 4*KPT FMAs; the per-CTA partial sums stay in registers across all its tiles and are added at the end into the fp64
+// accumulator of the launcher (acc64_*: the result does not depend on the order in which CTAs finish).
 template <int KPT>
 __global__ void __launch_bounds__(256)
-thin_wgrad2_kernel(const float* __restrict__ x, const float* __restrict__ dz, float* __restrict__ dwt, int N, int H, int W,
+thin_wgrad2_kernel(const float* __restrict__ x, const float* __restrict__ dz, double* __restrict__ dwt, int N, int H, int W,
                    int CinP, int OH, int OW, int Cout, int KH, int KW, int s, int pad, int pad_mode, int R, int tiles_w,
                    int tiles_h, int num_tiles, const float* __restrict__ relu_src, double* __restrict__ bias_sums) {
     extern __shared__ __align__(16) float sm[];
@@ -441,8 +441,9 @@ thin_wgrad2_kernel(const float* __restrict__ x, const float* __restrict__ dz, fl
     for (int i = 0; i < KPT; ++i) {
         const int k = cg * KPT + i;
         if (k < K) {
-            float* dst = dwt + (size_t)k * Cout + g * 4;
-            atomicAdd(dst, acc[i][0]); atomicAdd(dst + 1, acc[i][1]); atomicAdd(dst + 2, acc[i][2]); atomicAdd(dst + 3, acc[i][3]);
+            double* dst = dwt + (size_t)k * Cout + g * 4;
+            atomicAdd(dst, (double)acc[i][0]); atomicAdd(dst + 1, (double)acc[i][1]);
+            atomicAdd(dst + 2, (double)acc[i][2]); atomicAdd(dst + 3, (double)acc[i][3]);
         }
     }
     if (bias_sums && (256 % G) == 0) {
@@ -558,7 +559,7 @@ conv_img_dgrad_kernel(const float* __restrict__ dz4, const float* __restrict__ x
 }
 // dW[co][ci][tap] += sum_pix dz[pix][co] * act(x[pix+tap][ci]); db[co] += sum dz.  One block = 8x32 pixel tile.
 __global__ void __launch_bounds__(256)
-conv_img_wgrad_kernel(const float* __restrict__ dz4, const float* __restrict__ x, float* __restrict__ dw, float* __restrict__ db,
+conv_img_wgrad_kernel(const float* __restrict__ dz4, const float* __restrict__ x, double* __restrict__ dw, double* __restrict__ db,
                       int N, int H, int W, int Cin, int Cout, int act_in, int tiles_w, int tiles_h, int num_tiles) {
     extern __shared__ __align__(16) float sm[];
     const int PW = 34, PH = 10, NP = PW * PH;
@@ -567,7 +568,7 @@ conv_img_wgrad_kernel(const float* __restrict__ dz4, const float* __restrict__ x
     // thread -> (ci, tap group): Cin*9 products per co; threads = 256: each handles (ci = t % Cin, taps t/Cin .. step 256/Cin)
     const int ci = threadIdx.x % Cin, tg = threadIdx.x / Cin, tgn = 256 / Cin;
     // taps of this thread: tg, tg + tgn, tg + 2*tgn, ... (at most 5 for Cin <= 128); the accumulators are indexed by the UNROLLED
-    // slot j, never by the run-time tap (a run-time index put the whole array in local memory: 2.5 ms per call)
+    // slot j, never by the run-time tap (a run-time index would put the whole array in local memory)
     constexpr int kSlots = 5;
     float acc[kSlots][3];
 #pragma unroll
@@ -638,11 +639,11 @@ conv_img_wgrad_kernel(const float* __restrict__ dz4, const float* __restrict__ x
             if (t < 9) {
 #pragma unroll
                 for (int co = 0; co < 3; ++co)
-                    if (co < Cout) atomicAdd(dw + ((size_t)co * Cin + ci) * 9 + t, acc[j][co]);
+                    if (co < Cout) atomicAdd(dw + ((size_t)co * Cin + ci) * 9 + t, (double)acc[j][co]);
             }
         }
     }
-    if (threadIdx.x < Cout && db) atomicAdd(db + threadIdx.x, bacc[threadIdx.x]);
+    if (threadIdx.x < Cout && db) atomicAdd(db + threadIdx.x, (double)bacc[threadIdx.x]);
 }
 
 // ------------------------------------------------------------------------------------ Cin -> 1 conv backward
@@ -687,7 +688,7 @@ conv_to1_dgrad_kernel(const float* __restrict__ dl, const float* __restrict__ w,
 }
 // dw[ci][tap] += sum_pix dl[pix] * x[pix + tap][ci]; one warp per (tap, 128-channel slab), grid-stride over pixels
 __global__ void __launch_bounds__(256)
-conv_to1_wgrad_kernel(const float* __restrict__ dl, const float* __restrict__ x, float* __restrict__ dw, float* __restrict__ db,
+conv_to1_wgrad_kernel(const float* __restrict__ dl, const float* __restrict__ x, double* __restrict__ dw, double* __restrict__ db,
                       int N, int H, int W, int Cin, int KH, int KW, int pad, int OH, int OW) {
     const int tap = blockIdx.y;
     const int kh = tap / KW, kw = tap - kh * KW;
@@ -708,12 +709,12 @@ conv_to1_wgrad_kernel(const float* __restrict__ dl, const float* __restrict__ x,
             a[0] = fmaf(d, xv.x, a[0]); a[1] = fmaf(d, xv.y, a[1]); a[2] = fmaf(d, xv.z, a[2]); a[3] = fmaf(d, xv.w, a[3]);
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) atomicAdd(dw + (size_t)(g0 * 4 + i) * KH * KW + tap, a[i]);
+        for (int i = 0; i < 4; ++i) atomicAdd(dw + (size_t)(g0 * 4 + i) * KH * KW + tap, (double)a[i]);
     }
     if (tap == 0 && threadIdx.x == 0 && db) {
         float s = 0.f;
         for (long long o = p0; o < p1; ++o) s += dl[o];
-        atomicAdd(db, s);
+        atomicAdd(db, (double)s);
     }
 }
 
@@ -780,8 +781,9 @@ __global__ void reflect_pad_bwd_kernel(const float* __restrict__ dpad, float* __
         reinterpret_cast<float4*>(dx)[idx] = a;
     }
 }
-// bilinear (align_corners=False) backward: scatter with atomics (tiny tensors: reference-encoder tail)
-__global__ void resize_bilinear_bwd_kernel(const float* __restrict__ dout, float* __restrict__ din, int N, int H, int W, int C,
+// bilinear (align_corners=False) backward: scatter with fp64 atomics into the launcher's acc64 buffer (tiny tensors:
+// reference-encoder tail)
+__global__ void resize_bilinear_bwd_kernel(const float* __restrict__ dout, double* __restrict__ din, int N, int H, int W, int C,
                                            int OH, int OW) {
     const long long total = (long long)N * OH * OW * C;
     const float sh = (float)H / OH, sw = (float)W / OW;
@@ -797,11 +799,11 @@ __global__ void resize_bilinear_bwd_kernel(const float* __restrict__ dout, float
         const int y0 = (int)fy, x0 = (int)fx;
         const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
         const float ly = fy - y0, lx = fx - x0, d = dout[idx];
-        float* b = din + (size_t)n * H * W * C + c;
-        atomicAdd(b + ((size_t)y0 * W + x0) * C, d * (1.f - ly) * (1.f - lx));
-        atomicAdd(b + ((size_t)y0 * W + x1) * C, d * (1.f - ly) * lx);
-        atomicAdd(b + ((size_t)y1 * W + x0) * C, d * ly * (1.f - lx));
-        atomicAdd(b + ((size_t)y1 * W + x1) * C, d * ly * lx);
+        double* b = din + (size_t)n * H * W * C + c;
+        atomicAdd(b + ((size_t)y0 * W + x0) * C, (double)(d * (1.f - ly) * (1.f - lx)));
+        atomicAdd(b + ((size_t)y0 * W + x1) * C, (double)(d * (1.f - ly) * lx));
+        atomicAdd(b + ((size_t)y1 * W + x0) * C, (double)(d * ly * (1.f - lx)));
+        atomicAdd(b + ((size_t)y1 * W + x1) * C, (double)(d * ly * lx));
     }
 }
 // masked mean broadcast backward: out[p,c] = mean_c * mtag[p], mean_c = sum_q x[q,c]*mref[q] / max(cnt,1)
@@ -995,7 +997,15 @@ extern "C" int mg_thin_wgrad(const float* x, const float* dz, float* dwt, int N,
     int grid = num_sms();
     if (grid > num_tiles) grid = num_tiles;
     const int R = seg_resize > 0 ? seg_resize : 1;
-    cudaMemsetAsync(dwt, 0, (size_t)K * Cout * 4, ST(stream));
+    double* acc = nullptr;
+    int rc = acc64_alloc(&acc, (size_t)K * Cout, ST(stream));
+    if (rc) return rc;
+    // partial sums -> acc (fp64, order-independent) -> dwt
+    auto finish = [&](int rc0) {
+        if (!rc0) rc0 = acc64_fold(acc, dwt, (size_t)K * Cout, 0, ST(stream));
+        const int rc1 = acc64_free(acc, ST(stream));
+        return rc0 ? rc0 : rc1;
+    };
     // register-tiled kernel: Cout 64/128, columns per thread = ceil(K / (256 / (Cout/4)))
     const int CG = Cout == 64 || Cout == 128 ? 256 / (Cout / 4) : 0;
     const int kpt = CG ? (K + CG - 1) / CG : 0;
@@ -1011,8 +1021,8 @@ extern "C" int mg_thin_wgrad(const float* x, const float* dz, float* dwt, int N,
 #define MG_TW2(KP)                                                                                                              \
     do {                                                                                                                         \
         cudaError_t e = cudaFuncSetAttribute(thin_wgrad2_kernel<KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);     \
-        if (e != cudaSuccess) return set_error((int)e, "thin_wgrad2 attr: %s", cudaGetErrorString(e));                           \
-        thin_wgrad2_kernel<KP><<<grid, 256, smem, ST(stream)>>>(x, dz, dwt, N, H, W, CinP, OH, OW, Cout, KH, KW, stride, pad,    \
+        if (e != cudaSuccess) return finish(set_error((int)e, "thin_wgrad2 attr: %s", cudaGetErrorString(e)));                   \
+        thin_wgrad2_kernel<KP><<<grid, 256, smem, ST(stream)>>>(x, dz, acc, N, H, W, CinP, OH, OW, Cout, KH, KW, stride, pad,    \
                                                                 pad_mode, R, tiles_w, tiles_h, num_tiles, relu_src, bias_sums);   \
     } while (0)
         if (kpt <= 3) MG_TW2(3);
@@ -1020,18 +1030,19 @@ extern "C" int mg_thin_wgrad(const float* x, const float* dz, float* dwt, int N,
         else if (kpt <= 8) MG_TW2(8);
         else MG_TW2(13);
 #undef MG_TW2
-        return check_launch("mg_thin_wgrad");
+        return finish(check_launch("mg_thin_wgrad"));
     }
-    if (relu_src || bias_sums) return set_error(-4, "mg_thin_wgrad: the fused ReLU / bias-sum form needs the register-tiled kernel (Cout 64 | 128)");
-    if ((K + parts - 1) / parts > 64) return set_error(-3, "mg_thin_wgrad: K %d too large for %d parts", K, parts);
+    if (relu_src || bias_sums)
+        return finish(set_error(-4, "mg_thin_wgrad: the fused ReLU / bias-sum form needs the register-tiled kernel (Cout 64 | 128)"));
+    if ((K + parts - 1) / parts > 64) return finish(set_error(-3, "mg_thin_wgrad: K %d too large for %d parts", K, parts));
     const size_t smem = ((size_t)PH * PW * CinP + 128 * (size_t)Cout) * 4;
     cudaError_t e = cudaFuncSetAttribute(thin_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return set_error((int)e, "thin_wgrad attr: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return finish(set_error((int)e, "thin_wgrad attr: %s", cudaGetErrorString(e)));
     int grid2 = num_sms() * 2;
     if (grid2 > num_tiles) grid2 = num_tiles;
-    thin_wgrad_kernel<<<grid2, 256, smem, ST(stream)>>>(x, dz, dwt, N, H, W, CinP, OH, OW, Cout, KH, KW, stride, pad, pad_mode, R,
+    thin_wgrad_kernel<<<grid2, 256, smem, ST(stream)>>>(x, dz, acc, N, H, W, CinP, OH, OW, Cout, KH, KW, stride, pad, pad_mode, R,
                                                         tiles_w, tiles_h, num_tiles);
-    return check_launch("mg_thin_wgrad");
+    return finish(check_launch("mg_thin_wgrad"));
 }
 extern "C" int mg_thin_dgrad3(const float* dz, const float* wt, float* dimg_nchw, int N, int H, int W, int CinP, int OH, int OW, int Cout,
                               int KH, int KW, int stride, int pad, int c_lo, void* stream) {
@@ -1058,8 +1069,18 @@ extern "C" int mg_conv_img_bwd(const float* dy_nchw, const float* y_nchw, const 
     int grid = num_sms() * 2;
     if (grid > num_tiles) grid = num_tiles;
     const size_t smem = ((size_t)340 * (Cin + 1) + 256 * 4) * 4;
-    conv_img_wgrad_kernel<<<grid, 256, smem, ST(stream)>>>(dz4_ws, x, dw, db, N, H, W, Cin, Cout, act_in, tiles_w, tiles_h, num_tiles);
-    return check_launch("mg_conv_img_bwd");
+    // per-CTA partial sums -> fp64 (order-independent) -> added onto dw / db
+    const size_t n_dw = (size_t)Cout * Cin * 9, n_db = db ? (size_t)Cout : 0;
+    double* acc = nullptr;
+    int rc = acc64_alloc(&acc, n_dw + n_db, ST(stream));
+    if (rc) return rc;
+    conv_img_wgrad_kernel<<<grid, 256, smem, ST(stream)>>>(dz4_ws, x, acc, db ? acc + n_dw : nullptr, N, H, W, Cin, Cout, act_in,
+                                                           tiles_w, tiles_h, num_tiles);
+    rc = check_launch("mg_conv_img_bwd");
+    if (!rc) rc = acc64_fold(acc, dw, n_dw, 1, ST(stream));
+    if (!rc && db) rc = acc64_fold(acc + n_dw, db, n_db, 1, ST(stream));
+    const int rc2 = acc64_free(acc, ST(stream));
+    return rc ? rc : rc2;
 }
 extern "C" int mg_conv_to1_bwd(const float* dl, const float* x, const float* w, float* dx, float* dw, float* db, int N, int H, int W,
                                int Cin, int KH, int KW, int pad, int accumulate_dx, void* stream) {
@@ -1071,8 +1092,18 @@ extern "C" int mg_conv_to1_bwd(const float* dl, const float* x, const float* w, 
         count_launch();
     }
     if (dw) {
-        dim3 grid(num_sms() * 4, KH * KW);      // latency-bound per-thread pixel loops: 4x the blocks (was 0.5 ms per call)
-        conv_to1_wgrad_kernel<<<grid, 128, 0, ST(stream)>>>(dl, x, dw, db, N, H, W, Cin, KH, KW, pad, OH, OW);
+        // per-block partial sums -> fp64 (order-independent) -> added onto dw / db
+        const size_t n_dw = (size_t)Cin * KH * KW, n_db = db ? 1 : 0;
+        double* acc = nullptr;
+        int rc = acc64_alloc(&acc, n_dw + n_db, ST(stream));
+        if (rc) return rc;
+        dim3 grid(num_sms() * 4, KH * KW);      // latency-bound per-thread pixel loops: 4x the blocks
+        conv_to1_wgrad_kernel<<<grid, 128, 0, ST(stream)>>>(dl, x, acc, db ? acc + n_dw : nullptr, N, H, W, Cin, KH, KW, pad, OH, OW);
+        rc = check_launch("mg_conv_to1_bwd");
+        if (!rc) rc = acc64_fold(acc, dw, n_dw, 1, ST(stream));
+        if (!rc && db) rc = acc64_fold(acc + n_dw, db, n_db, 1, ST(stream));
+        const int rc2 = acc64_free(acc, ST(stream));
+        return rc ? rc : rc2;
     }
     return check_launch("mg_conv_to1_bwd");
 }
@@ -1088,8 +1119,15 @@ extern "C" int mg_reflect_pad_bwd(const float* dpad, float* dx, int N, int H, in
 }
 extern "C" int mg_resize_bilinear_bwd(const float* dout, float* din_zeroed, int N, int H, int W, int C, int OH, int OW, void* stream) {
     if (!dout || !din_zeroed) return set_error(-1, "mg_resize_bilinear_bwd: null pointer");
-    resize_bilinear_bwd_kernel<<<ew_grid_b((long long)N * OH * OW * C), 256, 0, ST(stream)>>>(dout, din_zeroed, N, H, W, C, OH, OW);
-    return check_launch("mg_resize_bilinear_bwd");
+    const size_t n = (size_t)N * H * W * C;
+    double* acc = nullptr;
+    int rc = acc64_alloc(&acc, n, ST(stream));
+    if (rc) return rc;
+    resize_bilinear_bwd_kernel<<<ew_grid_b((long long)N * OH * OW * C), 256, 0, ST(stream)>>>(dout, acc, N, H, W, C, OH, OW);
+    rc = check_launch("mg_resize_bilinear_bwd");
+    if (!rc) rc = acc64_fold(acc, din_zeroed, n, 1, ST(stream));
+    const int rc2 = acc64_free(acc, ST(stream));
+    return rc ? rc : rc2;
 }
 extern "C" int mg_masked_mean_bcast_bwd(const float* dout, const float* mref, const float* mtag, float* dx, int N, int h, int w, int C,
                                         int MH, int MW, void* stream) {

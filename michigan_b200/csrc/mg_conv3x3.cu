@@ -1,21 +1,18 @@
-// michigan_b200 — 3x3 / stride 1 / pad 1 implicit-GEMM convolution on tcgen05 with HALO patches and M-TILE GROUPS.
+// michigan_b200 — 3x3 / stride 1 / pad 1 implicit-GEMM convolution on wgmma with HALO patches and M-TILE GROUPS.
 //
 // Why a second kernel.  mg_igemm.cu loads one [128 px x 64 ch] activation box per (tap, K chunk) and streams the whole
 // weight operand once per 128-pixel tile: a 3x3 conv therefore pulls 9x its activations plus K*N weights per tile through
-// L2.  Measured on B200 the thin-N layers of the generator sit exactly on the L2->SM throughput cap (~6300 B/clk chip-wide):
-// up_3.conv_0 (128 -> 64 at 512^2, bf16 hi+lo) moves 17 GB per launch in 1.45 ms = 11.7 TB/s for 0.46 PFLOP of MMA work.
-// Here
+// L2: the thin-N layers of the generator (up_3.conv_0, 128 -> 64 at 512^2, bf16 hi+lo) move 17 GB per launch for
+// 0.46 PFLOP of MMA work.  Here
 //   * ONE [18 x 18 px x 128 B] activation patch per (K chunk, hi|lo part) serves all nine taps of TWO horizontally adjacent
-//     M tiles (8 x 16 pixels each) through UMMA descriptors whose start address is shifted by (kh*18 + kw + 8*mt) rows
+//     M tiles (8 x 16 pixels each) through wgmma descriptors whose start address is shifted by (kh*18 + kw + 8*mt) rows
 //     - activation traffic / 7.1;
 //   * every weight slot (one tap of one K chunk) is consumed by both M tiles before it is released - weight traffic / 2;
-//   * each M tile has its own MMA-issuing thread (the ~100-cycle issue floor per tcgen05.mma is per thread) and its own TMEM
-//     accumulator; with accumulators <= 128 columns the two groups in flight are double buffered (4 accumulators), so the
-//     epilogue of group g overlaps the MMAs of group g+1.
+//   * each consumer warpgroup keeps one register accumulator per M tile (2 x 64 registers at 128 columns).
 // Same operand formats (TF32 / fp16 / bf16, split precision merged or 3-pass), same epilogues (mg_epilogue.cuh), same
 // results as mg_igemm.cu up to accumulation order.
 //
-// Warp roles (384 threads): warp 0 TMA producer, warps 1 and 10 MMA issuers of M tile 0 / 1, warps 2..9 epilogue.
+// Warp roles (288 threads): warps 0..7 wgmma consumers (rows 0-63 / 64-127 of both M tiles) + epilogue, warp 8 TMA producer.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstring>
@@ -35,7 +32,7 @@ constexpr int kASlots = 2;
 
 struct Conv3Params {
     IgemmParams g;          // geometry, operand formats, epilogue (TW = 8, TH = 16, TN = 1)
-    int groups_w, num_groups, nbuf, b_slots, b_slot_bytes, steps_hi, steps_lo, n_items, bar3_off;
+    int groups_w, num_groups, b_slots, b_slot_bytes, steps_hi, steps_lo, n_items, bar3_off;
 };
 
 // item = (K chunk, activation part): part 0 = A (or A_hi), part 1 = A_lo.  Steps of an item = B slots it consumes:
@@ -53,37 +50,27 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     uint8_t* b_ring = smem + kASlots * kPatchBytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + q.bar3_off);
     uint64_t* bfull = bars;                         // [kMaxBSlots]
-    uint64_t* bempty = bars + kMaxBSlots;           // [kMaxBSlots], count kGM
+    uint64_t* bempty = bars + kMaxBSlots;           // [kMaxBSlots], one arrival per consumer warp
     uint64_t* afull = bars + 2 * kMaxBSlots;        // [kASlots]
-    uint64_t* aempty = afull + kASlots;             // [kASlots], count kGM
-    uint64_t* tfull = aempty + kASlots;             // [2 * kGM]
-    uint64_t* tempty = tfull + 2 * kGM;             // [2 * kGM], count 8 warps * 32
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2 * kGM);
+    uint64_t* aempty = afull + kASlots;             // [kASlots], one arrival per consumer warp
+    float* acc_tile = reinterpret_cast<float*>(smem + p.acc_off);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kNumEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmA2);
         tma_prefetch_desc(&tmB);
-        for (int s = 0; s < q.b_slots; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], kGM); }
-        for (int s = 0; s < kASlots; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], kGM); }
-        for (int a = 0; a < 2 * kGM; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], kNumEpiWarps * 32); }
+        for (int s = 0; s < q.b_slots; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], kNumEpiWarps); }
+        for (int s = 0; s < kASlots; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], kNumEpiWarps); }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int groups_per_img = q.groups_w * p.tiles_h;
     const bool split = p.parts > 1;
 
-    if (warp == 0) {
+    if (warp == kNumEpiWarps) {
         // ===================== TMA producer (one thread): A patches are issued one item ahead of the weight stream ===========
         if (lane == 0) {
             int bs = 0, as_ = 0;
@@ -134,79 +121,62 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                 }
             }
         }
-    } else if (warp == 1 || warp == 10) {
-        // ===================== MMA issuers: thread `mt` drives M tile `mt` of every group =====================
-        if (lane == 0) {
-            const int mt = warp == 1 ? 0 : 1;
-            const uint32_t a_base0 = smem_u32(a_ring), b_base0 = smem_u32(b_ring);
-            int bs = 0, as_ = 0, buf = 0;
-            uint32_t bph = 0, aphs = 0, tph = 0;
-            for (int gi = blockIdx.x; gi < q.num_groups; gi += gridDim.x) {
-                const int acc = buf * kGM + mt;
-                mbar_wait(&tempty[acc], tph ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.acc_cols);
-                for (int it = 0; it < q.n_items; ++it) {
-                    const int part = split ? (it & 1) : 0;
-                    const uint32_t idesc = (p.merged && part == 1) ? p.idesc2 : p.idesc;
-                    mbar_wait(&afull[as_], aphs);
-                    const uint32_t a_base = a_base0 + (uint32_t)(as_ * kPatchBytes);
-                    const int steps = part ? q.steps_lo : q.steps_hi;
-                    for (int st = 0; st < steps; ++st) {
-                        const int tap = steps == 18 ? (st >> 1) : st;
-                        const int kh = tap / 3, kw = tap - kh * 3;
-                        mbar_wait(&bfull[bs], bph);
-                        tc_fence_after();
-                        // tap (kh, kw) of M tile mt = the patch read from row kh*18 + kw + 8*mt on; 8-pixel row groups are 18 rows apart
-                        const uint32_t a_tap = a_base + (uint32_t)((kh * kPatchW + kw + 8 * mt) * 128);
-                        const uint64_t db = umma_desc_kmajor_sw128(b_base0 + (uint32_t)(bs * q.b_slot_bytes));
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t da = umma_desc_sw128_general(a_tap + (uint32_t)(k * 32), (uint32_t)(kPatchW * 128), 0u);
-                            const uint32_t accum = (it | st | k) != 0 ? 1u : 0u;
-                            if (p.a_fmt == 0) umma_tf32(d_tmem, da, db + (uint64_t)(2 * k), idesc, accum);
-                            else umma_f16(d_tmem, da, db + (uint64_t)(2 * k), idesc, accum);
-                        }
-                        umma_commit(&bempty[bs]);      // this issuer's reads of the slot are done when these MMAs retire
-                        if (++bs == q.b_slots) { bs = 0; bph ^= 1; }
-                    }
-                    umma_commit(&aempty[as_]);
-                    if (++as_ == kASlots) { as_ = 0; aphs ^= 1; }
-                }
-                umma_commit(&tfull[acc]);
-                if (++buf == q.nbuf) { buf = 0; tph ^= 1; }
-            }
-        }
-    } else if (warp >= 2 && warp < 2 + kNumEpiWarps) {
-        // ===================== epilogue warps: the two accumulators of a group, M tile 0 then 1 =====================
-        const int ew = warp - 2;
+    } else {
+        // ===================== consumers: warpgroup wg multiplies rows 64*wg.. of BOTH M tiles of a group, then all 8 warps
+        // run the epilogue of M tile 0 and of M tile 1
+        const int wg = warp >> 2;
         const int quarter = warp & 3;
-        const int half = ew >> 2;
-        float* scr = reinterpret_cast<float*>(smem + p.epi_off) + ew * (32 * (CW + 4));
-        int buf = 0;
-        uint32_t tph = 0;
+        const int half = warp >> 2;
+        float* scr = reinterpret_cast<float*>(smem + p.epi_off) + warp * (32 * (CW + 4));
+        const uint32_t a_base0 = smem_u32(a_ring), b_base0 = smem_u32(b_ring);
+        float acc0[64], acc1[64];
+        int bs = 0, as_ = 0;
+        uint32_t bph = 0, aphs = 0;
         for (int gi = blockIdx.x; gi < q.num_groups; gi += gridDim.x) {
             const int nt = gi % p.n_tiles;
             const int mg = gi / p.n_tiles;
             const int gw = mg % q.groups_w, th = (mg / q.groups_w) % p.tiles_h, tn = mg / groups_per_img;
-            for (int mt = 0; mt < kGM; ++mt) {
-                const int acc = buf * kGM + mt;
-                epilogue_tile<SPEC, CW>(p, scr, &tfull[acc], tph, tmem_base + (uint32_t)(acc * p.acc_cols), nt, gw * kGM + mt, th, tn,
-                                        quarter, half, lane, nullptr, p.epi_early ? &tempty[acc] : nullptr);
-                if (!p.epi_early) {
-                    tc_fence_before();
-                    mbar_arrive(&tempty[acc]);
+            for (int it = 0; it < q.n_items; ++it) {
+                const int part = split ? (it & 1) : 0;
+                const int n = (p.merged && part == 1) ? p.BN : p.acc_cols;
+                mbar_wait(&afull[as_], aphs);
+                // rows 64.. of an M tile are its pixel rows 8.., eight patch rows further on
+                const uint32_t a_base = a_base0 + (uint32_t)(as_ * kPatchBytes) + (uint32_t)(wg * 8 * kPatchW * 128);
+                const int steps = part ? q.steps_lo : q.steps_hi;
+                for (int st = 0; st < steps; ++st) {
+                    const int tap = steps == 18 ? (st >> 1) : st;
+                    const int kh = tap / 3, kw = tap - kh * 3;
+                    mbar_wait(&bfull[bs], bph);
+                    // tap (kh, kw) of M tile mt = the patch read from row kh*18 + kw + 8*mt on; 8-pixel row groups are 18 rows apart
+                    const uint32_t a_tap = a_base + (uint32_t)((kh * kPatchW + kw) * 128);
+                    const uint64_t db = wg_desc_sw128(b_base0 + (uint32_t)(bs * q.b_slot_bytes), 1024);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        const uint32_t accum = (it | st | k) != 0 ? 1u : 0u;
+                        const uint64_t da0 = wg_desc_sw128(a_tap + (uint32_t)(k * 32), (uint32_t)(kPatchW * 128));
+                        const uint64_t da1 = wg_desc_sw128(a_tap + (uint32_t)(8 * 128 + k * 32), (uint32_t)(kPatchW * 128));
+                        wgmma_k32b(acc0, n, p.a_fmt, da0, db + (uint64_t)(2 * k), accum);
+                        wgmma_k32b(acc1, n, p.a_fmt, da1, db + (uint64_t)(2 * k), accum);
+                    }
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&bempty[bs]);     // this warp's reads of the slot are done
+                    if (++bs == q.b_slots) { bs = 0; bph ^= 1; }
                 }
+                if (lane == 0) mbar_arrive(&aempty[as_]);
+                if (++as_ == kASlots) { as_ = 0; aphs ^= 1; }
             }
-            if (++buf == q.nbuf) { buf = 0; tph ^= 1; }
+            bar_sync(1, kNumEpiWarps * 32);
+            acc_store(acc_tile, p.acc_ld, acc0, p.acc_cols, wg * 64);
+            bar_sync(1, kNumEpiWarps * 32);
+            epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM, th, tn, quarter, half, lane);
+            bar_sync(1, kNumEpiWarps * 32);
+            acc_store(acc_tile, p.acc_ld, acc1, p.acc_cols, wg * 64);
+            bar_sync(1, kNumEpiWarps * 32);
+            epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM + 1, th, tn, quarter, half, lane);
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
     }
 }
 
@@ -214,12 +184,13 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
 // < 0 / > 0 on error.
 int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw, int scratch_bytes, int spec, cudaStream_t stream) {
     // eligibility: 3x3, stride 1, pad 1, same-size output, transposed epilogue, an even number of 8-pixel tile columns,
-    // at least 16 rows, and accumulators that fit TMEM twice over (one per M tile)
+    // and at least 16 rows
     if (!(a->KH == 3 && a->KW == 3 && a->stride == 1 && p.pad_h == 1 && p.pad_w == 1 && a->H == a->OH && a->W == a->OW && p.epi_impl == 1 &&
-          a->OW >= 16 && a->OW % 16 == 0 && a->OH >= 16 && p.os == 1 && p.acc_cols * kGM <= 512))
+          a->OW >= 16 && a->OW % 16 == 0 && a->OH >= 16 && p.os == 1))
         return 0;
+    const int acc_bytes = 128 * p.acc_ld * 4;
     {
-        const int avail0 = 227 * 1024 - 1024 - 512 - scratch_bytes - kASlots * kPatchBytes;
+        const int avail0 = 227 * 1024 - 1024 - 512 - scratch_bytes - acc_bytes - kASlots * kPatchBytes;
         if (avail0 / (p.acc_cols * 128) < 3) return 0;
     }
     Conv3Params q;
@@ -229,21 +200,21 @@ int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw,
     p.tiles_h = (a->OH + 15) / 16;
     p.tiles_n = a->N;
     p.num_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
-    p.halo = 0; p.dual = 0;
+    p.halo = 0;
     q.groups_w = p.tiles_w / kGM;
     q.num_groups = q.groups_w * p.tiles_h * p.tiles_n * p.n_tiles;
-    q.nbuf = (512 / p.acc_cols) / kGM >= 2 ? 2 : 1;
     const bool split = a->split != 0;
     q.steps_hi = (split && !p.merged) ? 18 : 9;
     q.steps_lo = 9;
     q.n_items = p.kchunks * (split ? 2 : 1);
     q.b_slot_bytes = p.acc_cols * 128;     // merged: [W_hi ; W_lo] = 2*BN rows; otherwise BN rows
-    const int avail = 227 * 1024 - 1024 - 512 - scratch_bytes - kASlots * kPatchBytes;
+    const int avail = 227 * 1024 - 1024 - 512 - scratch_bytes - acc_bytes - kASlots * kPatchBytes;
     q.b_slots = avail / q.b_slot_bytes;
     if (q.b_slots > kMaxBSlots) q.b_slots = kMaxBSlots;
     const size_t ring_bytes = (size_t)kASlots * kPatchBytes + (size_t)q.b_slots * q.b_slot_bytes;
     q.bar3_off = (int)ring_bytes;
     p.epi_off = (int)ring_bytes + 512;
+    p.acc_off = p.epi_off + scratch_bytes;
     p.parts = p.merged ? 2 : (split ? 3 : 1);
     q.g = p;
 
@@ -272,7 +243,7 @@ int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw,
         int rc = encode_tensor_map(&tmB, (void*)a->wpack, dt, 2, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
-    const size_t smem_bytes = ring_bytes + 1024 + 512 + scratch_bytes;
+    const size_t smem_bytes = ring_bytes + 1024 + 512 + scratch_bytes + acc_bytes;
     static thread_local int attr_set_dev = -1;
     int dev = 0;
     cudaGetDevice(&dev);

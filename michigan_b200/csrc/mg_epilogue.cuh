@@ -1,5 +1,5 @@
 // michigan_b200 — shared pieces of the implicit-GEMM convolution kernels: the parameter block and the transposed,
-// coalesced epilogue (TMEM accumulator tile -> bias / residual / blend / SPADE modulation -> global memory).
+// coalesced epilogue (accumulator tile in shared memory -> bias / residual / blend / SPADE modulation -> global memory).
 // Used by mg_igemm.cu (per-tap operand loads) and mg_conv3x3.cu (halo patches, M-tile groups).
 #pragma once
 #include <cuda.h>
@@ -12,9 +12,9 @@
 namespace mg {
 
 constexpr int kNumEpiWarps = 8;
-// warps 0/1: TMA producer + MMA issuer of pipeline 0, warps 2..9: epilogue, warps 10/11: producer + issuer of pipeline 1
-// (dual mode: the two pipelines work on alternate tiles / TMEM accumulators, see IgemmParams::dual)
-constexpr int kThreads = 64 + kNumEpiWarps * 32 + 64;  // 384
+// warps 0..7: two consumer warpgroups (wgmma on rows 0-63 / 64-127 of the 128-pixel tile, then the epilogue), warp 8: TMA producer
+constexpr int kThreads = kNumEpiWarps * 32 + 32;  // 288
+constexpr int kMaxAccCols = 128;                  // accumulator columns per tile: 64 fp32 registers per consumer thread
 constexpr int kABytes = 128 * 128;                // 128 pixels x 32 fp32
 constexpr int kMaxStages = 8;
 constexpr int kMaxASlots = 4;
@@ -25,7 +25,6 @@ struct IgemmParams {
     int os, ooh, oow, OHF, OWF, accumulate;
     int TW, TH, TN, tiles_w, tiles_h, tiles_n;
     int BN, n_tiles, num_tiles, kchunks, stages;
-    uint32_t idesc, tmem_cols;
     int epi, act, round_out;
     int a_fmt, parts, kelem;      // operand format: 0 tf32 (32 ch / 128 B row), 1 fp16, 2 bf16 (64 ch / row); parts 1 or 3
     float* out;                   // fp32 output (may be null when only 16-bit copies are wanted)
@@ -48,16 +47,10 @@ struct IgemmParams {
     const float* gbias1;
     const float* bbias;
     float* aux;   // SPADE: optional [N,OH,OW,Cout] copy of (1 + gamma) for the backward pass
-    int epi_early;                     // transposed epilogue releases the accumulator after its last TMEM read (MG_EPI_EARLY)
-    int epi_xpf;                       // TMA SPADE epilogue: prefetch x ahead of the accumulator wait (MG_EPI_TMA=2)
-    int epi_impl, epi_cw16, epi_off;   // 1 = transposed/coalesced epilogue (default), 2 = SPADE row-per-lane + TMA stores; scratch offset in smem
+    int epi_impl, epi_cw16, epi_off;   // 1 = transposed/coalesced epilogue (default), 0 = row-per-lane; scratch offset in smem
+    int acc_off, acc_ld;               // smem accumulator tile: byte offset, row pitch in floats (acc_cols + 4: conflict-free rows)
     // halo mode (3x3, stride 1, pad 1): one [PW x (TH+2)] input patch per K chunk serves all 9 taps
     int halo, PW, patch_bytes, patch_tx, a_slots, b_slots, b_slot_bytes, acc_cols, merged, n_items, bar_off;
-    uint32_t idesc2;
-    // dual mode: a single thread issues at most one tcgen05.mma per ~100-120 cycles whatever its N (microbenchmark
-    // profiles/r01_mma_rate_two_issuers.log: N=64 120 -> 62 cycles/MMA with two issuers, N=128 120 -> 85), so thin-N layers
-    // run two independent (producer, issuer) pairs, each with half of the stage ring and one of the two accumulators.
-    int dual, ring_stages;
     int dbg;   // what-if probes (env MG_DBG; 1..8 give WRONG results): 1 no B loads after the first tile, 2 no A loads, 4 no epilogue work, 8 no epilogue global traffic (32 no 16-bit stores only, 64 no x loads only), 16 cycle profile
 };
 
@@ -69,22 +62,18 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 }
 
 
-// One accumulator tile (128 pixels x BN columns at TMEM address t_acc) through the epilogue, executed by the 8 epilogue
-// warps together (warp -> TMEM lane quarter `quarter` = warp & 3 and column half `half`).  TMEM gives each lane one
+// One accumulator tile (128 pixels x BN columns, fp32 [128][ld] in shared memory) through the epilogue, executed by the 8
+// consumer warps together (warp -> row quarter `quarter` = warp & 3 and column half `half`).  Each lane reads one
 // accumulator ROW (pixel); the raw accumulators of a CW-channel chunk are dumped to a warp-private smem scratch `scr`
 // (32 x (CW + 4) floats) and read back transposed, so that in the arithmetic and in every global access a group of 4/8
 // lanes covers one pixel's contiguous channels (full 64/128 B segments) instead of 32 lanes touching 32 different lines.
-// The per-pixel bookkeeping is done BEFORE waiting on `tfull` (the accumulator-complete barrier).
 // SPEC selects a compile-time specialisation of the (instruction-bound) epilogue:
 //   0 generic (everything decided at run time)
 //   1 SPADE + LeakyReLU -> bf16 hi/lo operand only      2 SPADE + no activation -> bf16 hi/lo operand only
 // CW: channels per epilogue chunk (16 or 32), compile time so that the per-chunk register arrays are sized exactly.
 template <int SPEC, int CW>
-__device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, uint64_t* tfull, uint32_t parity, uint32_t t_acc,
-                                              int nt, int tw, int th, int tn, int quarter, int half, int lane, long long* w_tfull,
-                                              uint64_t* tempty = nullptr) {
-    // tempty != nullptr (IgemmParams::epi_early): this function releases the accumulator itself, right after the last TMEM
-    // read of the tile's last chunk instead of after its arithmetic and stores; the caller then must not arrive again.
+__device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, const float* acc, int nt, int tw, int th, int tn,
+                                              int quarter, int half, int lane) {
     constexpr bool kS = SPEC == 1 || SPEC == 2;
     const bool spade = kS ? true : (p.epi == 1);
     const int act = SPEC == 1 ? 2 : (SPEC == 2 ? 0 : p.act);
@@ -117,24 +106,12 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
         if (spade) srco[j] = (uint32_t)(((size_t)n * p.XH + (oh >> p.x_shift)) * p.XW + (ow >> p.x_shift));
         else if (p.res) srco[j] = (uint32_t)(((size_t)n * p.RH + (oh >> p.res_shift)) * p.RW + (ow >> p.res_shift));
     }
-    const long long t0 = w_tfull ? clock64() : 0;
-    mbar_wait(tfull, parity);
-    if (w_tfull) *w_tfull += clock64() - t0;
-    tc_fence_after();
-    const uint32_t t_row = t_acc + ((uint32_t)(quarter * 32) << 16);
-    bool released = tempty == nullptr;
+    const float* t_row = acc + (size_t)(quarter * 32 + lane) * p.acc_ld;
     for (int cb = 0; cb < span; cb += cw) {
         if (MG_DBGV(p) & 4) break;
-        const bool last_chunk = cb + cw >= span;
-        auto release = [&]() {
-            if (last_chunk && !released) { tc_fence_before(); mbar_arrive(tempty); released = true; }
-        };
         const int col = half * span + cb;          // first column of this chunk (gamma part for SPADE)
         float4 av[passes], bv[passes], pre[passes];
         const int cch = (spade ? nt * ch_tile : nt * p.BN) + col + q * 4;
-        // TMEM chunk -> registers: ALL tcgen05.ld of the chunk (gamma and beta halves) are issued back to back and
-        // waited for once - under a running MMA stream one ld+wait round trip costs ~1000 cycles, so the old
-        // load/wait-per-16-columns order serialised eight of them per tile.
         uint32_t g0[16], g1[16], b0[16], b1[16];
         // registers (row per lane) -> scratch -> registers (transposed: lanes cover contiguous channels)
         auto transpose = [&](const uint32_t (&v0)[16], const uint32_t (&v1)[16], float4 (&dst)[passes], bool add) {
@@ -160,19 +137,16 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
         };
         auto load_chunk = [&](int colbase, float4 (&dst)[passes], bool add) {
             uint32_t v0[16], v1[16];
-            tmem_ld16(t_row + (uint32_t)colbase, v0);
-            if (cw == 32) tmem_ld16(t_row + (uint32_t)(colbase + 16), v1);
-            tmem_ld_wait();
+            acc_ld16(t_row, colbase, v0);
+            if (cw == 32) acc_ld16(t_row, colbase + 16, v1);
             transpose(v0, v1, dst, add);
         };
-        tmem_ld16(t_row + (uint32_t)col, g0);
-        if (cw == 32) tmem_ld16(t_row + (uint32_t)(col + 16), g1);
+        acc_ld16(t_row, col, g0);
+        if (cw == 32) acc_ld16(t_row, col + 16, g1);
         if (spade) {
-            tmem_ld16(t_row + (uint32_t)(col + ch_tile), b0);
-            if (cw == 32) tmem_ld16(t_row + (uint32_t)(col + ch_tile + 16), b1);
+            acc_ld16(t_row, col + ch_tile, b0);
+            if (cw == 32) acc_ld16(t_row, col + ch_tile + 16, b1);
         }
-        tmem_ld_wait();
-        if (!p.merged) release();
         const bool ch_ok = cch < p.Cout;
         transpose(g0, g1, av, false);
         // Per-pixel side loads (SPADE: the tensor being normalised; else the residual): issued as soon as the first
@@ -183,7 +157,7 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
             for (int j = 0; j < passes; ++j)
                 if ((vmask >> j) & 1u) pre[j] = __ldg(reinterpret_cast<const float4*>(side + (size_t)srco[j] * p.Cout + cch));
         }
-        if (p.merged) { load_chunk(col + p.BN, av, true); if (!spade) release(); }   // split precision, merged N: + A_hi * W_lo columns
+        if (p.merged) load_chunk(col + p.BN, av, true);   // split precision, merged N: + A_hi * W_lo columns
         if (spade) transpose(b0, b1, bv, false);
         float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f), sc4 = bias4, sh4 = bias4, g14 = bias4, bb4 = bias4;
         if (ch_ok) {
@@ -208,7 +182,7 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
                 av[j] = make_float4(fmaf(xv.x, sc4.x, sh4.x) * gs.x, fmaf(xv.y, sc4.y, sh4.y) * gs.y,
                                     fmaf(xv.z, sc4.z, sh4.z) * gs.z, fmaf(xv.w, sc4.w, sh4.w) * gs.w);
             }
-            if (p.merged) { load_chunk(col + ch_tile + p.BN, bv, true); release(); }
+            if (p.merged) load_chunk(col + ch_tile + p.BN, bv, true);
         }
         if (!ch_ok) continue;
 #pragma unroll
@@ -285,113 +259,6 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
             }
         }
     }
-    if (!released) { tc_fence_before(); mbar_arrive(tempty); }
-}
-
-// SPADE -> bf16 hi/lo operand, row-per-lane + TMA stores (IgemmParams::epi_impl == 2; SPEC 1 LeakyReLU, SPEC 2 no activation):
-//     out = act( norm(x) * (1 + gamma) + beta ),  gamma | beta = this tile's accumulator halves
-// (reference: normalization.py:110-116 with the batch-norm folded into nscale/nshift, LeakyReLU 0.2 of architecture.py:85 for
-// norm_0 / norm_1, none for norm_s; x is read at half resolution when the block's 2x nearest upsample is folded, generator.py:72).
-// Preconditions (checked by the launcher): BN = 256 (gamma | beta halves of 128 columns, this warp owns 64 output channels),
-// tile 16 x 8 pixels of ONE image, plain output layout, no merged split.  The lane keeps its TMEM row = pixel; the 16-bit
-// results of a 32-channel group are laid down as [32 pixels][64 B] in the SWIZZLE_64B pattern (16-byte chunk c of row r at
-// c ^ ((r >> 1) & 3): conflict-free per 8 lanes) and one lane hands the two 2 KB boxes (hi, lo) to the TMA unit, which
-// writes whole sectors and clips what lies outside the image.  Against the transposed epilogue this drops the smem
-// transposition and every 8-byte global store (the SM -> L2 path moves ~1 request per 11 cycles whatever its size);
-// x is read row-per-lane (with the fused 2x upsampling only 8 distinct pixels per warp instruction).
-// `stage`: this warp's 4 KB staging buffer (512 B aligned); `pending`: a TMA store of this warp may still be reading it.
-template <int SPEC>
-__device__ __forceinline__ void epilogue_tile_spade_tma(const IgemmParams& p, uint8_t* stage, const CUtensorMap* tmHi, const CUtensorMap* tmLo,
-                                                        uint64_t* tfull, uint64_t* tempty, uint32_t parity, uint32_t t_acc, int nt, int tw,
-                                                        int th, int tn, int quarter, int half, int lane, bool& pending, long long* w_tfull) {
-    constexpr int act = SPEC == 1 ? 2 : 0;
-    const int ch_tile = p.BN >> 1;                      // 128
-    const int ow = tw * 16 + (lane & 15), oh = th * 8 + quarter * 2 + (lane >> 4);
-    const bool valid = ow < p.OW && oh < p.OH;
-    const float* xrow = p.x + ((size_t)((size_t)tn * p.XH + (oh >> p.x_shift)) * p.XW + (ow >> p.x_shift)) * p.Cout;
-    uint8_t* st_hi = stage;
-    uint8_t* st_lo = stage + 2048;
-    const int sw = (lane >> 1) & 3;
-    const bool xok = valid && !(MG_DBGV(p) & 64);
-    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    // x does not depend on the accumulator: with epi_xpf the lane's 128-byte x line of the first 32-channel group is pulled into L1
-    // BEFORE waiting for the tile and the second group's while the first is computed - the real loads then hit L1 instead of
-    // paying an L2 / DRAM round trip on the epilogue's critical path (a prefetch costs no registers)
-    const float* xg0 = xrow + nt * ch_tile + half * 64;
-    if (p.epi_xpf && xok) asm volatile("prefetch.global.L1 [%0];" :: "l"(xg0));
-    const long long t0 = w_tfull ? clock64() : 0;
-    mbar_wait(tfull, parity);
-    if (w_tfull) *w_tfull += clock64() - t0;
-    tc_fence_after();
-    const uint32_t t_row = t_acc + ((uint32_t)(quarter * 32) << 16);
-    bool released = false;
-#pragma unroll 1
-    for (int g = 0; g < 2; ++g) {
-        if (MG_DBGV(p) & 4) break;
-        const int col = half * 64 + g * 32;              // gamma column of this group inside the tile; beta at + ch_tile
-        const int cch = nt * ch_tile + col;              // output channel
-        uint32_t g0[16], g1[16], b0[16], b1[16];
-        tmem_ld16(t_row + (uint32_t)col, g0);
-        tmem_ld16(t_row + (uint32_t)(col + 16), g1);
-        tmem_ld16(t_row + (uint32_t)(col + ch_tile), b0);
-        tmem_ld16(t_row + (uint32_t)(col + ch_tile + 16), b1);
-        float4 xv[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) xv[i] = xok ? __ldg(reinterpret_cast<const float4*>(xrow + cch + 4 * i)) : zero4;
-        if (p.epi_xpf && xok && g == 0) asm volatile("prefetch.global.L1 [%0];" :: "l"(xg0 + 32));
-        tmem_ld_wait();
-        if (g == 1) {
-            // the last accumulator columns of this warp are in registers: hand the TMEM buffer back to the MMA issuer NOW, not
-            // after the second group's arithmetic and stores (role profile: the issuer spent 32 % of the kernel waiting for it)
-            tc_fence_before();
-            mbar_arrive(tempty);
-            released = true;
-        }
-        if (pending) { if (lane == 0) tma_store_wait_read(); __syncwarp(); pending = false; }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {                    // 16-byte chunk = 8 channels
-            const uint32_t* gv = c < 2 ? g0 : g1;
-            const uint32_t* bv = c < 2 ? b0 : b1;
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int h2 = 0; h2 < 2; ++h2) {
-                const int e = (c & 1) * 8 + h2 * 4;      // element inside the 16-column register array
-                const int ch = cch + c * 8 + h2 * 4;
-                const float4 sc = __ldg(reinterpret_cast<const float4*>(p.nscale + ch));
-                const float4 sh = __ldg(reinterpret_cast<const float4*>(p.nshift + ch));
-                const float4 g1b = __ldg(reinterpret_cast<const float4*>(p.gbias1 + ch));
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bbias + ch));
-                const float4 x4 = xv[c * 2 + h2];
-                float y[4];
-                y[0] = fmaf(x4.x, sc.x, sh.x) * (g1b.x + __uint_as_float(gv[e])) + (bb.x + __uint_as_float(bv[e]));
-                y[1] = fmaf(x4.y, sc.y, sh.y) * (g1b.y + __uint_as_float(gv[e + 1])) + (bb.y + __uint_as_float(bv[e + 1]));
-                y[2] = fmaf(x4.z, sc.z, sh.z) * (g1b.z + __uint_as_float(gv[e + 2])) + (bb.z + __uint_as_float(bv[e + 2]));
-                y[3] = fmaf(x4.w, sc.w, sh.w) * (g1b.w + __uint_as_float(gv[e + 3])) + (bb.w + __uint_as_float(bv[e + 3]));
-#pragma unroll
-                for (int i = 0; i < 4; ++i) y[i] = apply_act(y[i], act);
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const __nv_bfloat162 hh = __floats2bfloat162_rn(y[2 * i], y[2 * i + 1]);
-                    const float2 hf = __bfloat1622float2(hh);
-                    const __nv_bfloat162 ll = __floats2bfloat162_rn(y[2 * i] - hf.x, y[2 * i + 1] - hf.y);
-                    hi[h2 * 2 + i] = *reinterpret_cast<const uint32_t*>(&hh);
-                    lo[h2 * 2 + i] = *reinterpret_cast<const uint32_t*>(&ll);
-                }
-            }
-            const int off = lane * 64 + ((c ^ sw) << 4);
-            *reinterpret_cast<uint4*>(st_hi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4*>(st_lo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0 && !(MG_DBGV(p) & (8 | 32))) {
-            tma_store_4d(tmHi, st_hi, cch, tw * 16, th * 8 + quarter * 2, tn);
-            tma_store_4d(tmLo, st_lo, cch, tw * 16, th * 8 + quarter * 2, tn);
-            tma_store_commit();
-        }
-        pending = true;
-    }
-    if (!released) { tc_fence_before(); mbar_arrive(tempty); }
 }
 
 }  // namespace mg

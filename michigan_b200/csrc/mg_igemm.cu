@@ -1,4 +1,4 @@
-// michigan_b200 — im2col-free implicit-GEMM convolution on tcgen05 (sm_100a).
+// michigan_b200 — im2col-free implicit-GEMM convolution on wgmma (sm_90a).
 //
 //   D[pixels(128) x BN] += sum_{tap, cin-chunk} A_tap[pixels x 32] * W[BN x 32]^T
 //
@@ -6,10 +6,11 @@
 //   tap offset and TMA's out-of-bounds zero fill implements the conv zero padding; strided convs
 //   use the tensor map's elementStrides (traversal stride) so no im2col / space-to-depth copy exists;
 // * weights pre-packed tap-major [CoutG][KH*KW*Cin] and loaded by a 2-D TMA box;
-// * both operands land in 128B-swizzled K-major smem tiles that tcgen05.mma (kind::tf32) reads
-//   directly; fp32 accumulators live in TMEM, double buffered so the epilogue of tile i overlaps
-//   the main loop of tile i+1;
-// * warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc), warps 2..9 = epilogue;
+// * both operands land in 128B-swizzled K-major smem tiles that wgmma reads directly; the fp32
+//   accumulator lives in the registers of two consumer warpgroups (rows 0-63 / 64-127 of the tile)
+//   and goes through a shared-memory tile to the epilogue those same 8 warps run; the producer
+//   keeps filling the stage ring meanwhile;
+// * warp roles: warps 0..7 = wgmma consumers + epilogue, warp 8 = TMA producer;
 // * persistent CTAs (<= 1 per SM), static round-robin tile schedule with the N-tile index fastest
 //   so CTAs running concurrently share activation tiles through L2.
 //
@@ -28,7 +29,7 @@
 
 namespace mg {
 
-// MG_DBG & 16 (probe build): CTA 0 records clock64() totals here (see mg_debug_igemm_prof)
+// role-profile counters read by mg_debug_igemm_prof
 __device__ unsigned long long g_igemm_prof[16];
 
 // 16 consecutive channels -> 16-bit hi (and optional lo = cvt(y - hi)) copies, 32 B each.
@@ -67,8 +68,7 @@ __device__ __forceinline__ void store16(const IgemmParams& p, const float (&y)[1
 template <int SPEC, int CW>
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                  const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOHi,
-                  const __grid_constant__ CUtensorMap tmOLo, const IgemmParams p) {
+                  const __grid_constant__ CUtensorMap tmB, const IgemmParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // 1024-align the operand ring (SWIZZLE_128B atoms are 1024 B).
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -76,46 +76,33 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.bar_off);
     uint64_t* full_bar = bars;                        // halo mode: the weight (B) ring
     uint64_t* empty_bar = bars + kMaxStages;
-    uint64_t* tfull_bar = bars + 2 * kMaxStages;
-    uint64_t* tempty_bar = bars + 2 * kMaxStages + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
-    uint64_t* afull_bar = bars + 2 * kMaxStages + 5;  // halo mode: the patch (A) ring, <= kMaxASlots slots
+    uint64_t* afull_bar = bars + 2 * kMaxStages;      // halo mode: the patch (A) ring, <= kMaxASlots slots
     uint64_t* aempty_bar = afull_bar + kMaxASlots;
+    float* acc_tile = reinterpret_cast<float*>(smem + p.acc_off);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kNumEpiWarps && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmA2);
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < (p.halo ? p.b_slots : p.stages); ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], kNumEpiWarps);
         }
         for (int s = 0; s < p.a_slots; ++s) {
             mbar_init(&afull_bar[s], 1);
-            mbar_init(&aempty_bar[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tfull_bar[a], 1);
-            mbar_init(&tempty_bar[a], kNumEpiWarps * 32);
+            mbar_init(&aempty_bar[s], kNumEpiWarps);
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, p.tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int ksteps = p.KH * p.KW * p.parts * p.kchunks;
     const int m_tiles_per_img = p.tiles_w * p.tiles_h;
 
-    if (warp == 0 && p.halo) {
+    if (warp == kNumEpiWarps && p.halo) {
         // ===================== TMA producer, halo mode (one thread) =====================
         // Two rings: A = input patches (one per K chunk [x hi/lo part], reused by all 9 taps), B = weights
         // (one slot per tap).  A patches are prefetched up to a_slots-1 items ahead of the weight stream.
@@ -128,8 +115,6 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             uint32_t bph = 0, aphs = 0;
             long long a_issued = 0, b_item = 0;
             int tileA = blockIdx.x, itA = 0;
-            const bool prof = (MG_DBGV(p) & 16) && blockIdx.x == 0;
-            long long w_empty = 0, t_begin = prof ? clock64() : 0;
             for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
                 const int nt = tile % p.n_tiles;
                 for (int it = 0; it < p.n_items; ++it, ++b_item) {
@@ -149,9 +134,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             if (++itA == p.n_items) { itA = 0; tileA += gridDim.x; }
                             ++a_issued;
                         }
-                        const long long t0 = prof ? clock64() : 0;
                         mbar_wait(&empty_bar[bs], bph ^ 1);
-                        if (prof) w_empty += clock64() - t0;
                         uint8_t* sb = b_ring + (size_t)bs * p.b_slot_bytes;
                         const int kofs = tap * bparts * p.Cin + kc * p.kelem;
                         if (p.merged && part == 0) {
@@ -167,74 +150,13 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                 }
             }
-            if (prof) { g_igemm_prof[0] = (unsigned long long)(clock64() - t_begin); g_igemm_prof[1] = (unsigned long long)w_empty; }
         }
-    } else if (warp == 1 && p.halo) {
-        // ===================== MMA issuer, halo mode (one thread) =====================
+    } else if (warp == kNumEpiWarps) {
+        // ===================== TMA producer (one thread) =====================
         if (lane == 0) {
-            const int parts2 = p.merged ? 2 : 1;
-            const uint32_t a_ring = smem_u32(smem);
-            const uint32_t b_ring = a_ring + (uint32_t)(p.a_slots * p.patch_bytes);
-            int bs = 0, as_ = 0, acc = 0;
-            uint32_t bph = 0, aphs = 0, aph = 0;
-            const bool prof = (MG_DBGV(p) & 16) && blockIdx.x == 0;
-            long long w_tempty = 0, w_full = 0, t_begin = prof ? clock64() : 0;
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                long long t0 = prof ? clock64() : 0;
-                mbar_wait(&tempty_bar[acc], aph ^ 1);
-                if (prof) w_tempty += clock64() - t0;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.acc_cols);
-                for (int it = 0; it < p.n_items; ++it) {
-                    const int part = it % parts2;
-                    const uint32_t idesc = (p.merged && part == 1) ? p.idesc2 : p.idesc;
-                    t0 = prof ? clock64() : 0;
-                    mbar_wait(&afull_bar[as_], aphs);
-                    if (prof) w_full += clock64() - t0;
-                    const uint32_t a_base = a_ring + (uint32_t)(as_ * p.patch_bytes);
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const int kh = tap / 3, kw = tap - kh * 3;
-                        t0 = prof ? clock64() : 0;
-                        mbar_wait(&full_bar[bs], bph);
-                        if (prof) w_full += clock64() - t0;
-                        tc_fence_after();
-                        // tap (kh, kw) = the same patch read from row kh*PW + kw on; 8-pixel row groups are PW rows apart
-                        const uint32_t a_tap = a_base + (uint32_t)((kh * p.PW + kw) * 128);
-                        const uint64_t db = umma_desc_kmajor_sw128(b_ring + (uint32_t)(bs * p.b_slot_bytes));
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint32_t a_addr = a_tap + (uint32_t)(k * 32);
-                            const uint64_t da = umma_desc_sw128_general(a_addr, (uint32_t)(p.PW * 128), 0u);
-                            const uint32_t accum = (it | tap | k) != 0 ? 1u : 0u;
-                            if (p.a_fmt == 0) umma_tf32(d_tmem, da, db + (uint64_t)(2 * k), idesc, accum);
-                            else umma_f16(d_tmem, da, db + (uint64_t)(2 * k), idesc, accum);
-                        }
-                        umma_commit(&empty_bar[bs]);
-                        if (++bs == p.b_slots) { bs = 0; bph ^= 1; }
-                    }
-                    umma_commit(&aempty_bar[as_]);
-                    if (++as_ == p.a_slots) { as_ = 0; aphs ^= 1; }
-                }
-                umma_commit(&tfull_bar[acc]);
-                if (++acc == 2) { acc = 0; aph ^= 1; }
-            }
-            if (prof) {
-                g_igemm_prof[2] = (unsigned long long)(clock64() - t_begin);
-                g_igemm_prof[3] = (unsigned long long)w_tempty; g_igemm_prof[4] = (unsigned long long)w_full;
-            }
-        }
-    } else if (warp == 0 || (p.dual && warp == 10)) {
-        // ===================== TMA producer (one thread per pipeline) =====================
-        if (lane == 0) {
-            const int pipe = warp == 10 ? 1 : 0, npipes = p.dual ? 2 : 1;
-            uint64_t* const full_bar_p = full_bar + pipe * p.ring_stages;
-            uint64_t* const empty_bar_p = empty_bar + pipe * p.ring_stages;
-            uint8_t* const ring = smem + (size_t)pipe * p.ring_stages * stage_bytes;
             int st = 0;
             uint32_t ph = 0;
-            const bool prof = (MG_DBGV(p) & 16) && blockIdx.x == 0 && pipe == 0;
-            long long w_empty = 0, t_begin = prof ? clock64() : 0;
-            for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += npipes * gridDim.x) {
+            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
                 const bool ldA = !(MG_DBGV(p) & 2) || tile == (int)blockIdx.x, ldB = !(MG_DBGV(p) & 1) || tile == (int)blockIdx.x;
                 const int nt = tile % p.n_tiles;
                 const int m = tile / p.n_tiles;
@@ -254,167 +176,106 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const int bsel = part == 2 ? 1 : 0;
                         const bool both = p.merged && part == 0;
                         for (int kc = 0; kc < p.kchunks; ++kc) {
-                            const long long t0 = prof ? clock64() : 0;
-                            mbar_wait(&empty_bar_p[st], ph ^ 1);
-                            if (prof) w_empty += clock64() - t0;
-                            uint8_t* sa = ring + (size_t)st * stage_bytes;
+                            mbar_wait(&empty_bar[st], ph ^ 1);
+                            uint8_t* sa = smem + (size_t)st * stage_bytes;
                             const uint32_t txs = (ldA ? kABytes : 0) + (ldB ? p.BN * 128 * (both ? 2 : 1) : 0);
-                            if (txs == 0) { mbar_arrive(&full_bar_p[st]); }
-                            else mbar_arrive_expect_tx(&full_bar_p[st], txs);
-                            if (ldA) tma_load_4d(sa, ta, &full_bar_p[st], kc * p.kelem, iw0 + kw, ih0 + kh, n0);
+                            if (txs == 0) { mbar_arrive(&full_bar[st]); }
+                            else mbar_arrive_expect_tx(&full_bar[st], txs);
+                            if (ldA) tma_load_4d(sa, ta, &full_bar[st], kc * p.kelem, iw0 + kw, ih0 + kh, n0);
                             const int kofs = (tap * bparts + bsel) * p.Cin + kc * p.kelem;
                             if (ldB) {
-                                tma_load_2d(sa + kABytes, &tmB, &full_bar_p[st], kofs, nt * p.BN);
-                                if (both) tma_load_2d(sa + kABytes + p.BN * 128, &tmB, &full_bar_p[st], kofs + p.Cin, nt * p.BN);
+                                tma_load_2d(sa + kABytes, &tmB, &full_bar[st], kofs, nt * p.BN);
+                                if (both) tma_load_2d(sa + kABytes + p.BN * 128, &tmB, &full_bar[st], kofs + p.Cin, nt * p.BN);
                             }
-                            if (++st == p.ring_stages) { st = 0; ph ^= 1; }
+                            if (++st == p.stages) { st = 0; ph ^= 1; }
                         }
                     }
                 }
             }
-            if (prof) { g_igemm_prof[0] = (unsigned long long)(clock64() - t_begin); g_igemm_prof[1] = (unsigned long long)w_empty; }
         }
-    } else if (warp == 1 || (p.dual && warp == 11)) {
-        // ===================== MMA issuer (one thread per pipeline) =====================
-        if (lane == 0) {
-            const int pipe = warp == 11 ? 1 : 0, npipes = p.dual ? 2 : 1;
-            uint64_t* const full_bar_p = full_bar + pipe * p.ring_stages;
-            uint64_t* const empty_bar_p = empty_bar + pipe * p.ring_stages;
-            const uint32_t ring = smem_u32(smem) + (uint32_t)(pipe * p.ring_stages * stage_bytes);
-            int st = 0;
-            uint32_t ph = 0;
-            int acc = pipe;            // dual: pipeline j owns accumulator j; single: the accumulators alternate
-            uint32_t aph = 0;
-            const bool prof = (MG_DBGV(p) & 16) && blockIdx.x == 0 && pipe == 0;
-            long long w_tempty = 0, w_full = 0, t_begin = prof ? clock64() : 0;
-            for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += npipes * gridDim.x) {
-                long long t0 = prof ? clock64() : 0;
-                mbar_wait(&tempty_bar[acc], aph ^ 1);
-                if (prof) w_tempty += clock64() - t0;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.acc_cols);
-                for (int ks = 0; ks < ksteps; ++ks) {
-                    t0 = prof ? clock64() : 0;
-                    mbar_wait(&full_bar_p[st], ph);
-                    if (prof) w_full += clock64() - t0;
-                    tc_fence_after();
-                    const uint32_t sa = ring + (uint32_t)(st * stage_bytes);
-                    const uint64_t da = umma_desc_kmajor_sw128(sa);
-                    const uint64_t db = umma_desc_kmajor_sw128(sa + kABytes);
-                    // merged split precision: k-steps alternate (per K-chunk run) between N = 2*BN and N = BN
-                    const uint32_t idesc = (p.merged && ((ks / p.kchunks) & 1)) ? p.idesc2 : p.idesc;
+    } else {
+        // ===================== consumers: warpgroup wg multiplies rows 64*wg.. of the tile, then all 8 warps run the epilogue
+        const int wg = warp >> 2;
+        const int quarter = warp & 3;           // rows 32*quarter.. of the accumulator tile in the epilogue
+        const int half = warp >> 2;             // column half handled by this warp in the epilogue
+        float* scr = reinterpret_cast<float*>(smem + p.epi_off) + warp * (32 * (CW + 4));
+        float acc[64];
+        int st = 0, bs = 0, as_ = 0;
+        uint32_t ph = 0, bph = 0, aphs = 0;
+        const uint32_t ring = smem_u32(smem);
+        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+            const int nt = tile % p.n_tiles;
+            const int m = tile / p.n_tiles;
+            const int tw = m % p.tiles_w;
+            const int th = (m / p.tiles_w) % p.tiles_h;
+            const int tn = m / m_tiles_per_img;
+            if (p.halo) {
+                const int parts2 = p.merged ? 2 : 1;
+                const uint32_t b_ring = ring + (uint32_t)(p.a_slots * p.patch_bytes);
+                for (int it = 0; it < p.n_items; ++it) {
+                    const int part = it % parts2;
+                    const int n = (p.merged && part == 1) ? p.BN : p.acc_cols;
+                    mbar_wait(&afull_bar[as_], aphs);
+                    // rows 64.. of the tile are its pixel rows 8.., eight patch rows of PW pixels further on
+                    const uint32_t a_base = ring + (uint32_t)(as_ * p.patch_bytes) + (uint32_t)(wg * 8 * p.PW * 128);
+                    for (int tap = 0; tap < 9; ++tap) {
+                        const int kh = tap / 3, kw = tap - kh * 3;
+                        mbar_wait(&full_bar[bs], bph);
+                        // tap (kh, kw) = the same patch read from row kh*PW + kw on; 8-pixel row groups are PW rows apart
+                        const uint32_t a_tap = a_base + (uint32_t)((kh * p.PW + kw) * 128);
+                        const uint64_t db = wg_desc_sw128(b_ring + (uint32_t)(bs * p.b_slot_bytes), 1024);
+                        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        // advance 8 tf32 = 32 B inside the 128 B swizzle row: +2 in 16 B units
-                        if (p.a_fmt == 0)
-                            umma_tf32(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (ks | k) != 0 ? 1u : 0u);
-                        else
-                            umma_f16(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (ks | k) != 0 ? 1u : 0u);
+                        for (int k = 0; k < 4; ++k) {
+                            const uint64_t da = wg_desc_sw128(a_tap + (uint32_t)(k * 32), (uint32_t)(p.PW * 128));
+                            wgmma_k32b(acc, n, p.a_fmt, da, db + (uint64_t)(2 * k), (it | tap | k) != 0 ? 1u : 0u);
+                        }
+                        wgmma_commit();
+                        wgmma_wait_all();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty_bar[bs]);
+                        if (++bs == p.b_slots) { bs = 0; bph ^= 1; }
                     }
-                    umma_commit(&empty_bar_p[st]);  // frees the smem stage when these MMAs retire
-                    if (++st == p.ring_stages) { st = 0; ph ^= 1; }
+                    if (lane == 0) mbar_arrive(&aempty_bar[as_]);
+                    if (++as_ == p.a_slots) { as_ = 0; aphs ^= 1; }
                 }
-                umma_commit(&tfull_bar[acc]);  // accumulator complete -> epilogue
-                if (p.dual) aph ^= 1;
-                else if (++acc == 2) { acc = 0; aph ^= 1; }
+            } else {
+                for (int ks = 0; ks < ksteps; ++ks) {
+                    mbar_wait(&full_bar[st], ph);
+                    const uint32_t sa = ring + (uint32_t)(st * stage_bytes);
+                    const uint64_t da = wg_desc_sw128(sa + (uint32_t)(wg * 64 * 128), 1024);
+                    const uint64_t db = wg_desc_sw128(sa + kABytes, 1024);
+                    // merged split precision: k-steps alternate (per K-chunk run) between N = 2*BN and N = BN
+                    const int n = (p.merged && ((ks / p.kchunks) & 1)) ? p.BN : p.acc_cols;
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)   // advance 32 B inside the 128 B swizzle row: +2 in 16 B units
+                        wgmma_k32b(acc, n, p.a_fmt, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (ks | k) != 0 ? 1u : 0u);
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[st]);   // this warp's reads of the stage are done
+                    if (++st == p.stages) { st = 0; ph ^= 1; }
+                }
             }
-            if (prof) {
-                g_igemm_prof[2] = (unsigned long long)(clock64() - t_begin);
-                g_igemm_prof[3] = (unsigned long long)w_tempty; g_igemm_prof[4] = (unsigned long long)w_full;
+            bar_sync(1, kNumEpiWarps * 32);     // the previous tile's epilogue is done with the accumulator tile
+            acc_store(acc_tile, p.acc_ld, acc, p.acc_cols, wg * 64);
+            bar_sync(1, kNumEpiWarps * 32);
+            if (p.epi_impl == 1) {
+                epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, tw, th, tn, quarter, half, lane);
+                continue;
             }
-        }
-    } else if (warp >= 2 && warp < 2 + kNumEpiWarps && p.epi_impl == 1) {
-        // ===================== epilogue warps: transposed, coalesced (mg_epilogue.cuh) =====================
-        const int ew = warp - 2;
-        const int quarter = warp & 3;
-        const int half = ew >> 2;
-        float* scr = reinterpret_cast<float*>(smem + p.epi_off) + ew * (32 * (CW + 4));
-        int acc = 0;
-        uint32_t aph = 0;
-        const bool prof = (MG_DBGV(p) & 16) && blockIdx.x == 0 && (ew == 0 || ew == 7) && lane == 0;
-        long long w_tfull = 0, t_begin = prof ? clock64() : 0;
-        int ntile = 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            const int nt = tile % p.n_tiles;
-            const int m = tile / p.n_tiles;
-            const int tw = m % p.tiles_w;
-            const int th = (m / p.tiles_w) % p.tiles_h;
-            const int tn = m / m_tiles_per_img;
-            epilogue_tile<SPEC, CW>(p, scr, &tfull_bar[acc], aph, tmem_base + (uint32_t)(acc * p.acc_cols), nt, tw, th, tn, quarter, half,
-                                    lane, prof ? &w_tfull : nullptr, p.epi_early ? &tempty_bar[acc] : nullptr);
-            if (!p.epi_early) {
-                tc_fence_before();
-                mbar_arrive(&tempty_bar[acc]);
-            }
-            ++ntile;
-            if (++acc == 2) { acc = 0; aph ^= 1; }
-        }
-        if (prof) {
-            const int o = ew == 0 ? 5 : 9;
-            const long long total = clock64() - t_begin;
-            g_igemm_prof[o] = (unsigned long long)total; g_igemm_prof[o + 1] = (unsigned long long)w_tfull;
-            g_igemm_prof[o + 2] = (unsigned long long)(total - w_tfull); g_igemm_prof[o + 3] = (unsigned long long)ntile;
-        }
-    } else if (warp >= 2 && warp < 2 + kNumEpiWarps && p.epi_impl == 2) {
-        // ===================== epilogue warps: SPADE -> bf16 hi/lo, row-per-lane + TMA stores (mg_epilogue.cuh) ===============
-        if constexpr (SPEC == 1 || SPEC == 2) {
-            const int ew = warp - 2;
-            const int quarter = warp & 3;
-            const int half = ew >> 2;
-            uint8_t* stage = smem + p.epi_off + ew * 4096;
-            int acc = 0;
-            uint32_t aph = 0;
-            bool pending = false;
-            const bool prof = (MG_DBGV(p) & 16) && blockIdx.x == 0 && (ew == 0 || ew == 7) && lane == 0;
-            long long w_tfull = 0, t_begin = prof ? clock64() : 0;
-            int ntile = 0;
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                const int nt = tile % p.n_tiles;
-                const int m = tile / p.n_tiles;
-                const int tw = m % p.tiles_w;
-                const int th = (m / p.tiles_w) % p.tiles_h;
-                const int tn = m / m_tiles_per_img;
-                epilogue_tile_spade_tma<SPEC>(p, stage, &tmOHi, &tmOLo, &tfull_bar[acc], &tempty_bar[acc], aph,
-                                              tmem_base + (uint32_t)(acc * p.acc_cols), nt, tw, th, tn, quarter, half, lane, pending,
-                                              prof ? &w_tfull : nullptr);      // releases the accumulator itself
-                ++ntile;
-                if (++acc == 2) { acc = 0; aph ^= 1; }
-            }
-            if (lane == 0) tma_store_wait_all();
-            if (prof) {
-                const int o = ew == 0 ? 5 : 9;
-                const long long total = clock64() - t_begin;
-                g_igemm_prof[o] = (unsigned long long)total; g_igemm_prof[o + 1] = (unsigned long long)w_tfull;
-                g_igemm_prof[o + 2] = (unsigned long long)(total - w_tfull); g_igemm_prof[o + 3] = (unsigned long long)ntile;
-            }
-        }
-    } else if (warp >= 2 && warp < 2 + kNumEpiWarps) {
-        // ===================== epilogue warps (row-per-lane reference implementation) =====================
-        const int ew = warp - 2;
-        const int quarter = warp & 3;           // TMEM lane quarter this warp may access
-        const int half = ew >> 2;               // column half handled by this warp
-        const int r = quarter * 32 + lane;      // accumulator row == pixel within tile
-        const int wl = r % p.TW;
-        const int hl = (r / p.TW) % p.TH;
-        const int nl = r / (p.TW * p.TH);
-        int acc = 0;
-        uint32_t aph = 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            const int nt = tile % p.n_tiles;
-            const int m = tile / p.n_tiles;
-            const int tw = m % p.tiles_w;
-            const int th = (m / p.tiles_w) % p.tiles_h;
-            const int tn = m / m_tiles_per_img;
+            // ===================== row-per-lane reference epilogue =====================
+            const int r = quarter * 32 + lane;      // accumulator row == pixel within tile
+            const int wl = r % p.TW;
+            const int hl = (r / p.TW) % p.TH;
+            const int nl = r / (p.TW * p.TH);
             const int ow = tw * p.TW + wl;
             const int oh = th * p.TH + hl;
             const int n = tn * p.TN + nl;
             const bool valid = (ow < p.OW) && (oh < p.OH) && (n < p.N);
             const size_t pix = ((size_t)n * p.OHF + (size_t)oh * p.os + p.ooh) * p.OWF + (size_t)ow * p.os + p.oow;
-
-            mbar_wait(&tfull_bar[acc], aph);
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * p.BN);
-
+            const float* t_row = acc_tile + (size_t)r * p.acc_ld;
             if (p.epi == 0) {
                 const int cols_half = p.BN >> 1;
                 float ps = 1.f, pm = 1.f, om_hair = 0.f, om_back = 1.f;
@@ -433,8 +294,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     resp = p.res + (((size_t)n * p.RH + (oh >> p.res_shift)) * p.RW + (ow >> p.res_shift)) * p.Cout;
                 for (int j0 = half * cols_half; j0 < (half + 1) * cols_half; j0 += 16) {
                     uint32_t v[16];
-                    tmem_ld16(t_row + j0, v);
-                    tmem_ld_wait();
+                    acc_ld16(t_row, j0, v);
                     const int c0 = nt * p.BN + j0;
                     if (valid && c0 < p.Cout) {
                         float y[16];
@@ -497,9 +357,8 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     xp = p.x + (((size_t)n * p.XH + (oh >> p.x_shift)) * p.XW + (ow >> p.x_shift)) * p.Cout;
                 for (int j0 = half * ch_half; j0 < (half + 1) * ch_half; j0 += 16) {
                     uint32_t g[16], b[16];
-                    tmem_ld16(t_row + j0, g);
-                    tmem_ld16(t_row + ch_tile + j0, b);
-                    tmem_ld_wait();
+                    acc_ld16(t_row, j0, g);
+                    acc_ld16(t_row, ch_tile + j0, b);
                     const int c0 = nt * ch_tile + j0;
                     if (valid && c0 < p.Cout) {
                         float y[16];
@@ -533,17 +392,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                 }
             }
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[acc]);
-            if (++acc == 2) { acc = 0; aph ^= 1; }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, p.tmem_cols);
     }
 }
 
@@ -564,22 +413,21 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
     if (a->out_hi && (a->out16_fmt < 1 || a->out16_fmt > 2)) return set_error(-11, "mg_conv_igemm: out16_fmt must be 1 or 2");
     if (a->out_lo && !a->out_hi) return set_error(-12, "mg_conv_igemm: out_lo without out_hi");
     const int coutg = a->epi == MG_EPI_SPADE ? 2 * a->Cout : a->Cout;
-    int BN = a->BN;
-    if (BN == 0) {
-        BN = coutg >= 256 ? 256 : coutg;
-        if (a->epi == MG_EPI_SPADE && BN < 64) BN = 64;
-    }
+    // BN: 32, 64 or 128 accumulator columns (the wgmma N of the consumer warpgroups; 128 keeps the accumulator at 64 registers
+    // per thread and its smem tile at 66 KB).  A wider request is narrowed.
+    int BN = a->BN == 0 || a->BN > kMaxAccCols ? kMaxAccCols : a->BN;
+    while (BN > 32 && coutg % BN != 0) BN /= 2;
     if (a->BN == 0 && a->epi != MG_EPI_SPADE && tune(TK_BN_FILL)) {
-        // Under-filled grids (the 8x8 .. 32x32 layers: 1024 -> 1024 at 8x8 is 4 pixel tiles x 4 column tiles = 16 CTAs on 148
-        // SMs): halve BN while twice as many tiles still fit one wave.  Thinner tiles cost MMA efficiency, idle SMs cost more
-        // (head_0.conv_0: 198 us on 16 CTAs).  The weight operand layout does not depend on BN.
+        // Under-filled grids (the 8x8 .. 32x32 layers: 1024 -> 1024 at 8x8 is 4 pixel tiles x 8 column tiles = 32 CTAs on 132
+        // SMs): halve BN while twice as many tiles still fit one wave.  Thinner tiles cost MMA efficiency, idle SMs cost more.
+        // The weight operand layout does not depend on BN.
         const int tw = next_pow2(a->OW) < 16 ? next_pow2(a->OW) : 16;
         const int th = next_pow2(a->OH) < 128 / tw ? next_pow2(a->OH) : 128 / tw;
         const int tn = 128 / (tw * th);
         const long long m_tiles = (long long)((a->OW + tw - 1) / tw) * ((a->OH + th - 1) / th) * ((a->N + tn - 1) / tn);
         while (BN > 64 && coutg % (BN / 2) == 0 && m_tiles * (coutg / BN) * 2 <= num_sms()) BN /= 2;
     }
-    if (BN % 32 != 0 || BN < 32 || BN > 256) return set_error(-3, "mg_conv_igemm: bad BN %d", BN);
+    if (BN != 32 && BN != 64 && BN != 128) return set_error(-3, "mg_conv_igemm: bad BN %d", BN);
     if (coutg % BN != 0) return set_error(-4, "mg_conv_igemm: GEMM N %d not a multiple of BN %d", coutg, BN);
     if (a->epi == MG_EPI_SPADE && (BN % 64 != 0 || !a->x || !a->nscale || !a->nshift || !a->gbias1 || !a->bbias))
         return set_error(-5, "mg_conv_igemm: SPADE epilogue needs x/nscale/nshift/gbias1/bbias and BN%%64==0");
@@ -598,32 +446,27 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
     const int epi_impl_env = a->epi == MG_EPI_SPADE ? tune(TK_EPI_IMPL_SPADE) : tune(TK_EPI_IMPL);
     // epilogue chunk width: 16 channels (no register spills) unless MG_EPI_CW16=0 / MG_EPI_CW_SPADE=32 ask for 32
     const int epi_cw16_env = tune(TK_EPI_CW16);
-    p.epi_impl = epi_impl_env; p.epi_cw16 = epi_cw16_env; p.epi_early = tune(TK_EPI_EARLY) ? 1 : 0;
-    // epilogue chunk width (channels per TMEM->scratch->register round): 16 everywhere by default (no register spills,
-    // 20 KB of scratch => one more pipeline stage at BN = 256); MG_EPI_CW16=0 / MG_EPI_CW_SPADE=32 select 32 where possible.
+    p.epi_impl = epi_impl_env; p.epi_cw16 = epi_cw16_env;
+    // epilogue chunk width (channels per accumulator->scratch->register round): 16 everywhere by default (no register spills,
+    // 20 KB of scratch); MG_EPI_CW16=0 / MG_EPI_CW_SPADE=32 select 32 where possible.
     const int span_epi = a->epi == MG_EPI_SPADE ? (BN >> 2) : (BN >> 1);
     const int cw_spade = tune(TK_CW_SPADE);
     int cw = (span_epi % 32 == 0 && !p.epi_cw16) ? 32 : 16;
     if (a->epi == MG_EPI_SPADE) cw = (cw_spade == 32 && span_epi % 32 == 0) ? 32 : 16;
     int scratch_bytes = p.epi_impl == 1 ? kNumEpiWarps * 32 * (cw + 4) * 4 : 0;
     // Halo mode: 3x3 / stride 1 / pad 1 convolutions (the SPADE gamma|beta GEMMs, conv_0/conv_1 and their dgrads) load
-    // one [PW x (TH+2)] input patch per K chunk and read the 9 taps out of it through shifted UMMA descriptors.
-    // MG_HALO: 0 off (default: measured no faster on B200 - these kernels are bound by the MMA operand fetch / epilogue,
-    // not by L2->smem traffic, see profiles/r01_prof_conv_*.log), 1 on; MG_HALO_PW: patch pitch in pixels (10 = exact, 16 = swizzle-atom aligned rows);
-    // (The descriptor's matrix-base-offset field must stay 0: measured on B200, the hardware applies the 128B swizzle on
-    // absolute shared-memory address bits; deriving the field from the start address gives wrong results.)
+    // one [PW x (TH+2)] input patch per K chunk and read the 9 taps out of it through shifted wgmma descriptors.
+    // MG_HALO: 0 off (default), 1 on; MG_HALO_PW: patch pitch in pixels (10 = exact, 16 = swizzle-atom aligned rows).
     const int halo_env = tune(TK_HALO);
     const int halo_pw = tune(TK_HALO_PW);
     bool halo = halo_env && p.epi_impl == 1 && a->KH == 3 && a->KW == 3 && a->stride == 1 && p.pad_h == 1 && p.pad_w == 1 &&
                 a->OH >= 16 && a->OW >= 8 && a->H == a->OH && a->W == a->OW && (halo_pw == 10 || halo_pw == 16);
     // merged split precision: A_hi x [W_hi ; W_lo] (N = 2*BN) + A_lo x W_hi (N = BN): two MMAs per K step instead of
-    // three (every tcgen05.mma costs >= ~100 cycles whatever its N, profiles/r01_mma_rate_microbench.log); the
-    // accumulator is 2*BN columns wide and the epilogue adds the halves.  MG_MERGE=0 restores the 3-pass form.
+    // three; the accumulator is 2*BN columns wide and the epilogue adds the halves.  MG_MERGE=0 restores the 3-pass form.
+    // Only where 2*BN still fits the accumulator.
     const int merge_env = tune(TK_MERGE);
     bool merged = false;
-    // Only where the GEMM N is thin anyway (<= 128): for wider layers three N = 256 passes beat two passes over
-    // twice as many N = 128 tiles (measured: 512->512 at 64^2 0.39 ms 3-pass vs 0.52 ms merged).
-    if (a->split && merge_env && p.epi_impl == 1 && BN <= 128) merged = true;
+    if (a->split && merge_env && p.epi_impl == 1 && 2 * BN <= kMaxAccCols) merged = true;
     if (halo && a->split && !merged) halo = false;
     p.halo = halo ? 1 : 0;
     p.merged = merged ? 1 : 0;
@@ -644,19 +487,13 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
     p.a_fmt = a->a_fmt; p.parts = merged ? 2 : (a->split ? 3 : 1); p.kelem = kelem;
     p.out_hi = a->out_hi; p.out_lo = a->out_lo; p.out16_fmt = a->out16_fmt;
     p.acc_cols = p.merged ? 2 * BN : BN;
-    // SPADE -> bf16 hi/lo operand at BN = 256 (the dominant GEMMs of the forward): row-per-lane epilogue that leaves through
-    // smem staging + TMA stores (epilogue_tile_spade_tma); 32 KB of staging instead of 20 KB of transposition scratch still
-    // leaves room for the 4-stage ring.  MG_EPI_TMA=0 keeps the transposed epilogue.
-    const bool tma_epi = tune(TK_EPI_TMA) && p.epi_impl == 1 && a->epi == MG_EPI_SPADE && !a->out && a->out_hi && a->out_lo &&
-                         a->out16_fmt == 2 && !a->aux_out && !a->round_out && (a->act == MG_ACT_LRELU || a->act == MG_ACT_NONE) && !merged &&
-                         !halo && BN == 256 && a->Cout % 32 == 0 && p.TW == 16 && p.TH == 8 && p.TN == 1 && p.os == 1 &&
-                         p.OHF == a->OH && p.OWF == a->OW && tune(TK_GROUP3) < 2;
-    if (tma_epi) { p.epi_impl = 2; p.epi_xpf = tune(TK_EPI_TMA) >= 2 ? 1 : 0; scratch_bytes = kNumEpiWarps * 4096; }
 #ifdef MG_PROBES
     p.dbg = probe_bits();
 #endif
     const int stage_bytes = kABytes + p.acc_cols * 128;
-    const int smem_avail = 227 * 1024 - 1024 - 512 - scratch_bytes;
+    p.acc_ld = p.acc_cols + 4;
+    const int acc_bytes = 128 * p.acc_ld * 4;
+    const int smem_avail = 227 * 1024 - 1024 - 512 - scratch_bytes - acc_bytes;
     size_t ring_bytes = 0;
     if (halo) {
         p.PW = halo_pw;
@@ -681,24 +518,10 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
         if (stages_cap > 0 && stages > stages_cap) stages = stages_cap;
         p.stages = stages;
         ring_bytes = (size_t)stages * stage_bytes;
-        // dual pipelines for thin N (one issuing thread cannot feed the tensor pipe below N = 256); MG_DUAL=0 disables
-        // MG_DUAL=2 (default since round 2: parity-checked, -5 % on the forward) also splits N = 256 layers, whose ring is then
-        // only 2 + 2 stages deep; MG_DUAL=1 keeps those on one pipeline
-        const int dual_env = tune(TK_DUAL);
-        const int sms = num_sms();
-        const int dual_cols = dual_env >= 2 ? 256 : 128;
-        if (dual_env && p.acc_cols <= dual_cols && stages >= 4 && p.num_tiles >= 2 * (a->max_ctas > 0 && a->max_ctas < sms ? a->max_ctas : sms)) {
-            p.dual = 1;
-            p.ring_stages = stages / 2;
-        }
     }
-    if (!p.dual) p.ring_stages = p.stages;
     p.bar_off = (int)ring_bytes;
     p.epi_off = (int)ring_bytes + 512;
-    p.idesc2 = a->a_fmt == 0 ? umma_idesc_tf32(128, BN) : umma_idesc_16(128, BN, a->a_fmt);
-    p.idesc = a->a_fmt == 0 ? umma_idesc_tf32(128, p.acc_cols) : umma_idesc_16(128, p.acc_cols, a->a_fmt);
-    int tc = next_pow2(2 * p.acc_cols);
-    p.tmem_cols = tc < 32 ? 32 : tc;
+    p.acc_off = p.epi_off + scratch_bytes;
     p.epi = a->epi; p.act = a->act; p.round_out = a->round_out;
     p.out = a->out; p.bias = a->bias;
     p.res = a->res; p.res_shift = a->res_shift;
@@ -714,10 +537,10 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
         !a->round_out && (a->act == MG_ACT_LRELU || a->act == MG_ACT_NONE))
         spec = a->act == MG_ACT_LRELU ? 1 : 2;
     // 3x3 / stride 1 / pad 1 layers: the halo-patch + M-tile-group kernel (mg_conv3x3.cu) moves 3-5x fewer bytes through L2.
-    // MG_GROUP3: 0 off, 1 (default) where its accumulators can be double buffered (<= 128 columns), 2 every eligible layer.
+    // MG_GROUP3: 0 off, 1 or 2 (default 1) every eligible layer.
     {
         const int g3 = tune(TK_GROUP3);
-        if (!halo && g3 && (g3 >= 2 || p.acc_cols <= 128)) {
+        if (!halo && g3) {
             IgemmParams p3 = p;
             const int rc3 = conv3x3_group_launch(a, p3, BN, cw, scratch_bytes, spec, stream);
             if (rc3 == 1) return 0;
@@ -750,19 +573,7 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
         int rc = encode_tensor_map(&tmB, (void*)a->wpack, dt, 2, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
-
-    CUtensorMap tmOHi = tmA, tmOLo = tmA;
-    if (p.epi_impl == 2) {
-        // [N][OH][OW][Cout] bf16; box = 32 channels x 16 x 2 pixels (one epilogue warp's quarter of a tile, 64-byte rows)
-        cuuint64_t dims[4] = {(cuuint64_t)a->Cout, (cuuint64_t)a->OW, (cuuint64_t)a->OH, (cuuint64_t)a->N};
-        cuuint64_t strides[3] = {(cuuint64_t)a->Cout * 2, (cuuint64_t)a->OW * a->Cout * 2, (cuuint64_t)a->OH * a->OW * a->Cout * 2};
-        cuuint32_t box[4] = {32, 16, 2, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        int rc = encode_tensor_map(&tmOHi, a->out_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
-        if (!rc) rc = encode_tensor_map(&tmOLo, a->out_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
-        if (rc) return rc;
-    }
-    const size_t smem_bytes = ring_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + scratch_bytes;
+    const size_t smem_bytes = ring_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + scratch_bytes + acc_bytes;
     static thread_local int attr_set_dev = -1;
     int dev = 0;
     cudaGetDevice(&dev);
@@ -778,7 +589,7 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
     int grid = num_sms();
     if (a->max_ctas > 0 && a->max_ctas < grid) grid = a->max_ctas;
     if (grid > p.num_tiles) grid = p.num_tiles;
-#define MG_LAUNCH(S, C) igemm_tf32_kernel<S, C><<<grid, kThreads, smem_bytes, stream>>>(tmA, tmA2, tmB, tmOHi, tmOLo, p)
+#define MG_LAUNCH(S, C) igemm_tf32_kernel<S, C><<<grid, kThreads, smem_bytes, stream>>>(tmA, tmA2, tmB, p)
     if (spec == 1) { if (cw == 32) MG_LAUNCH(1, 32); else MG_LAUNCH(1, 16); }
     else if (spec == 2) { if (cw == 32) MG_LAUNCH(2, 32); else MG_LAUNCH(2, 16); }
     else { if (cw == 32) MG_LAUNCH(0, 32); else MG_LAUNCH(0, 16); }
@@ -791,9 +602,7 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
 
 }  // namespace mg
 
-// Debug: copy the 16 clock64() counters CTA 0 recorded during the last launch made with MG_DBG&16 (synchronises).
-// [0] producer total, [1] producer wait-empty, [2] MMA total, [3] MMA wait-tmem-empty, [4] MMA wait-full,
-// [5..8] epilogue warp 0: total, wait-tmem-full, busy, tiles; [9..12] same for epilogue warp 7.
+// Debug: copy the 16 role-profile counters (synchronises).  The sm_90 kernel records none: all zero.
 extern "C" int mg_debug_igemm_prof(unsigned long long* host16) {
     if (!host16) return mg::set_error(-1, "mg_debug_igemm_prof: null pointer");
     cudaError_t e = cudaDeviceSynchronize();

@@ -1,4 +1,4 @@
-// michigan_b200 — internal helpers shared by the translation units of libmichigan_sm100.so.
+// michigan_b200 — internal helpers shared by the translation units of libmichigan_sm90.so.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -17,8 +17,8 @@ int encode_tensor_map(CUtensorMap* map, void* gaddr, CUtensorMapDataType dtype, 
 // Tuning knobs (alternative schedules that all give the same results): read ONCE from the environment at first use,
 // overridable through mg_set_tuning() (tests, A/B tools).  Nothing on the launch path calls getenv.
 enum TuneKnob {
-    TK_DUAL = 0,         // MG_DUAL: 0 one (producer, issuer) pipeline, 1 two for accumulators <= 128 columns, 2 (default) also for 256
-    TK_MERGE,            // MG_MERGE: split-precision convs with N <= 128 as two MMAs per K step (default 1)
+    TK_DUAL = 0,         // MG_DUAL: accepted, no effect on sm_90a
+    TK_MERGE,            // MG_MERGE: split-precision convs with 2*BN <= 128 as two MMAs per K step (default 1)
     TK_HALO,             // MG_HALO: halo schedule of 3x3/s1 convs (default 0)
     TK_HALO_PW,          // MG_HALO_PW: patch pitch 10 | 16
     TK_EPI_IMPL,         // MG_EPI_IMPL: 1 transposed epilogue (default), 0 row-per-lane reference epilogue
@@ -26,21 +26,21 @@ enum TuneKnob {
     TK_EPI_CW16,         // MG_EPI_CW16: 16-channel epilogue chunks (default 1)
     TK_CW_SPADE,         // MG_EPI_CW_SPADE: 16 | 32
     TK_STAGES,           // MG_STAGES: cap on the smem ring depth (0 = none)
-    TK_WGRAD_DUAL,       // MG_WGRAD_DUAL (default 1)
+    TK_WGRAD_DUAL,       // MG_WGRAD_DUAL: accepted, no effect on sm_90a
     TK_THIN_GEMM,        // MG_THIN_GEMM (default 1)
     TK_THIN_WGRAD_LEGACY,// MG_THIN_WGRAD_LEGACY (default 0)
-    TK_GROUP3,           // MG_GROUP3: 3x3/s1 convs on the halo-patch + M-tile-group kernel (mg_conv3x3.cu): 0 off, 1 thin N, 2 all
+    TK_GROUP3,           // MG_GROUP3: 3x3/s1 convs on the halo-patch + M-tile-group kernel (mg_conv3x3.cu): 0 off, 1 / 2 on
     TK_SEG_TMA,          // MG_SEG_TMA: 16-bit outputs of the seg conv through smem staging + TMA stores (default 1)
-    TK_WGRAD_HALO,       // MG_WGRAD_HALO: bf16 stride-1 weight gradients load one input patch per stage for all KW taps (default 1)
-    TK_EPI_TMA,          // MG_EPI_TMA: SPADE -> bf16 hi/lo epilogue at BN 256 row-per-lane through smem staging + TMA stores (default 1)
+    TK_WGRAD_HALO,       // MG_WGRAD_HALO: accepted, no effect on sm_90a
+    TK_EPI_TMA,          // MG_EPI_TMA: accepted, no effect on sm_90a
     TK_BN_FILL,          // MG_BN_FILL: generic convs whose tiles do not fill the SMs use a narrower BN (default 1)
-    TK_EPI_EARLY,        // MG_EPI_EARLY: transposed epilogue hands the accumulator back after its last TMEM read (default 0: not yet measured)
+    TK_EPI_EARLY,        // MG_EPI_EARLY: accepted, no effect on sm_90a
     TK_COUNT
 };
 int tune(int knob);
 
 // What-if probes (skip loads / epilogue work: WRONG results, timing experiments only) and the clock64() role profile exist
-// only in a library built with -DMG_PROBES (python -m michigan_b200.build --probes -> libmichigan_sm100_probes.so);
+// only in a library built with -DMG_PROBES (python -m michigan_b200.build --probes -> libmichigan_sm90_probes.so);
 // the product library compiles them out.
 #ifdef MG_PROBES
 int probe_bits();   // env MG_DBG, read once
@@ -54,6 +54,14 @@ int probe_bits();   // env MG_DBG, read once
 struct IgemmParams;
 // mg_conv3x3.cu: 1 = launched, 0 = shape not eligible (use the per-tap kernel), anything else = error status
 int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw, int scratch_bytes, int spec, cudaStream_t stream);
+
+// Order-independent reductions.  Kernels whose CTAs add partial sums into the same elements in whatever order they finish
+// accumulate into a zeroed fp64 buffer instead of the fp32 destination: sums of fp32 partials of the magnitudes met here are
+// exact in fp64, so the result no longer depends on the finishing order and two runs on the same inputs agree bit for bit.
+// acc64_fold then writes dst[i] = (add ? dst[i] : 0) + (float)acc[i].  All three are stream-ordered.
+int acc64_alloc(double** acc, size_t n, cudaStream_t stream);
+int acc64_fold(const double* acc, float* dst, size_t n, int add, cudaStream_t stream);
+int acc64_free(double* acc, cudaStream_t stream);
 
 inline int check_launch(const char* what) {
     count_launch();

@@ -1,4 +1,4 @@
-// michigan_b200 — loss reductions of the train step (sm_100a).
+// michigan_b200 — loss reductions of the train step (sm_90a).
 //
 // The reference evaluates its adversarial losses as chains of small eager ops per discriminator scale
 // (models/networks/loss.py:60-78,100-140: interpolate -> 2x max_pool2d -> interpolate -> clamp -> mul -> mean;
@@ -62,7 +62,7 @@ struct LossTerm {
 };
 
 // grid.x blocks per term: terms range from 9 K (coarse logits) to 34 M elements (finest feature map) - enough blocks to saturate
-// HBM on the large ones (32 blocks per term measured 2.9 ms per call); blocks beyond a small term's size exit immediately
+// HBM on the large ones; blocks beyond a small term's size exit immediately
 constexpr int kLossBlocksPerTerm = 592;
 
 __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __restrict__ terms, double* __restrict__ slots) {

@@ -1,4 +1,4 @@
-// michigan_b200 — one-shot small all-reduce over NVLink peer memory (sm_100a).
+// michigan_b200 — one-shot small all-reduce over NVLink peer memory (sm_90a).
 //
 // The SyncBN statistics exchange of the reference (batchnorm.py:105-126: every replica sends [sum | sum of squares]
 // to the master through Python queues, comm.py:49-133; the master reduce-adds and broadcasts mean / inv_std) is a

@@ -5,8 +5,9 @@
 // the row  [ hi(36) | lo(36) | hi(36) | 0(20) ]  down in the 128B-swizzled K-major operand layout; the resident weight
 // operand is  [ W_hi | W_hi | W_lo | 0 ]  per output channel, so that the single accumulation
 //     A_hi.W_hi + A_lo.W_hi + A_hi.W_lo      (~16 significand bits, same split as the other bf16x3 convs)
-// comes out of 8 tcgen05.mma (M 128, N 128, K 16).  Warp roles: warp 0 = weights TMA + MMA issue, warps 1-4 = operand
-// builders (one pixel row each), warps 5-12 = epilogue (TMEM -> transposed through smem -> bias/ReLU -> coalesced stores).
+// comes out of 8 wgmma K steps (M 64 per warpgroup, N 128, K 16).  Warp roles: warps 0-7 = two consumer warpgroups (wgmma on
+// pixel rows 0-63 / 64-127, accumulator -> smem tile -> bias/ReLU -> coalesced stores), warps 8-11 = operand builders (one
+// pixel row each).
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -19,7 +20,8 @@
 
 namespace mg {
 
-constexpr int kSegThreads = 32 * 13;
+constexpr int kSegThreads = 32 * 12;
+constexpr int kSegAccLd = 132;             // row pitch (floats) of the [128 x 128] accumulator tile
 constexpr int kSegTileBytes = 2 * 16384;   // [128 rows x 128 K] bf16 as two K64 chunks of [128 x 128 B]
 
 // MG_DBG & 16: clock64() totals of CTA 0 (read back with mg_debug_seg_prof)
@@ -34,7 +36,6 @@ struct SegParams {
     int out16_fmt, round_out, act;
     int N, OH, OW, R;
     int tiles_w, tiles_h, num_tiles;
-    uint32_t idesc;
     int tma_store;   // 16-bit outputs leave through smem staging + TMA stores (out == null)
     int prof, dbg;   // dbg (MG_DBG bits, timing only): 1 no global stores, 2 no smem transposition
 };
@@ -53,67 +54,185 @@ seg_mlp_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     uint8_t* a_s = smem + kSegTileBytes;                    // 2 operand buffers
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 3 * kSegTileBytes);
     uint64_t* a_full = bars;          // [2] 128 builder threads
-    uint64_t* a_empty = bars + 2;     // [2] tcgen05.commit
-    uint64_t* t_full = bars + 4;      // [2] tcgen05.commit
-    uint64_t* t_empty = bars + 6;     // [2] 256 epilogue threads
-    uint64_t* w_full = bars + 8;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-    float* scratch = reinterpret_cast<float*>(smem + 3 * kSegTileBytes + 1024);   // 1024-aligned: also the TMA-store staging
+    uint64_t* a_empty = bars + 2;     // [2] 8 consumer warps
+    uint64_t* w_full = bars + 4;
+    // fp32 [128][kSegAccLd] accumulator tile (1024-aligned); once a warp's columns are in registers its 8 KB share is also
+    // that warp's TMA-store staging buffer
+    float* acc_tile = reinterpret_cast<float*>(smem + 3 * kSegTileBytes + 1024);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmW);
         for (int i = 0; i < 2; ++i) {
             mbar_init(&a_full[i], 128);
-            mbar_init(&a_empty[i], 1);
-            mbar_init(&t_full[i], 1);
-            mbar_init(&t_empty[i], 256);
+            mbar_init(&a_empty[i], 8);
         }
         mbar_init(w_full, 1);
         fence_barrier_init();
     }
-    if (warp == 0) { tmem_alloc(tmem_slot, 256); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int tiles_per_img = p.tiles_w * p.tiles_h;
 
-    if (warp == 0) {
-        // ===================== weights + MMA issue (one thread) =====================
-        if (lane == 0) {
+    if (warp < 8) {
+        // ===================== consumers: wgmma (warpgroup wg = pixel rows 64*wg..), then the epilogue of 8 warps =====================
+        if (warp == 0 && lane == 0) {
             mbar_arrive_expect_tx(w_full, kSegTileBytes);
             tma_load_2d(w_s, &tmW, w_full, 0, 0);
             tma_load_2d(w_s + 16384, &tmW, w_full, 64, 0);
-            mbar_wait(w_full, 0);
-            int it = 0;
-            const bool prof = MG_PROFV(p) && blockIdx.x == 0;
-            long long w_te = 0, w_af = 0, t_begin = prof ? clock64() : 0;
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-                const int s = it & 1;
-                const uint32_t ph = (uint32_t)(it >> 1) & 1u;
-                long long t0 = prof ? clock64() : 0;
-                mbar_wait(&t_empty[s], ph ^ 1);
-                if (prof) { const long long t1 = clock64(); w_te += t1 - t0; t0 = t1; }
-                mbar_wait(&a_full[s], ph);
-                if (prof) w_af += clock64() - t0;
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(a_s + (size_t)s * kSegTileBytes), w_addr = smem_u32(w_s);
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const uint64_t da = umma_desc_kmajor_sw128(a_addr + c * 16384), db = umma_desc_kmajor_sw128(w_addr + c * 16384);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_f16(tmem_base + (uint32_t)(s * 128), da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), p.idesc, (c | k) != 0 ? 1u : 0u);
-                }
-                umma_commit(&a_empty[s]);
-                umma_commit(&t_full[s]);
-            }
-            if (prof) { g_seg_prof[0] = (unsigned long long)(clock64() - t_begin); g_seg_prof[1] = (unsigned long long)w_te; g_seg_prof[2] = (unsigned long long)w_af; }
         }
-    } else if (warp <= 4) {
+        mbar_wait(w_full, 0);
+        const int wg = warp >> 2;
+        const int quarter = warp & 3, half = warp >> 2, ew = warp;
+        const int q = lane & 7, psub = lane >> 3;   // 8 lanes per pixel (32 channels), 4 pixels per pass
+        // this warp's [32 px][64 ch] share of the accumulator tile, read transposed by the fp32 / register-store epilogue
+        const float* scr = acc_tile + (size_t)(quarter * 32) * kSegAccLd + half * 64;
+        float acc[64];
+        int it = 0;
+        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+            const int s = it & 1;
+            const uint32_t ph = (uint32_t)(it >> 1) & 1u;
+            const int n = tile / tiles_per_img, m = tile - n * tiles_per_img;
+            const int oh0 = (m / p.tiles_w) * 8, ow0 = (m % p.tiles_w) * 16;
+            mbar_wait(&a_full[s], ph);
+            const uint32_t a_addr = smem_u32(a_s + (size_t)s * kSegTileBytes) + (uint32_t)(wg * 64 * 128), w_addr = smem_u32(w_s);
+            wgmma_fence();
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const uint64_t da = wg_desc_sw128(a_addr + c * 16384, 1024), db = wg_desc_sw128(w_addr + c * 16384, 1024);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_bf16_n128(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (c | k) != 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&a_empty[s]);
+            // the previous tile's epilogue reads (and TMA stores out of the staging buffers) are done with the tile
+            if (p.tma_store && it > 0) { if (lane == 0) tma_store_wait_read(); __syncwarp(); }
+            bar_sync(1, 256);
+            acc_store(acc_tile, kSegAccLd, acc, 128, wg * 64);
+            bar_sync(1, 256);
+            if (p.tma_store) {
+                // 16-bit outputs only: lane = pixel row of a [32 px][64 ch] box (two image rows of the tile).  Each lane lays its
+                // 128-byte row down in the SWIZZLE_128B pattern (16-byte chunk c at c ^ (row & 7): conflict-free per 8 lanes) and
+                // one lane hands the 4 KB box to the TMA unit, which writes whole lines and clips the part outside the image.
+                uint32_t v0[16], v1[16], v2[16], v3[16];
+                const float* arow = acc_tile + (size_t)(quarter * 32 + lane) * kSegAccLd + half * 64;
+                acc_ld16(arow, 0, v0); acc_ld16(arow, 16, v1); acc_ld16(arow, 32, v2); acc_ld16(arow, 48, v3);
+                bar_sync(1, 256);
+                uint8_t* st_hi = reinterpret_cast<uint8_t*>(acc_tile) + ew * 8192;
+                uint8_t* st_lo = st_hi + 4096;
+                const float* bsrc = p.bias + half * 64;
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    const uint32_t* v = (c >> 1) == 0 ? v0 : (c >> 1) == 1 ? v1 : (c >> 1) == 2 ? v2 : v3;
+                    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bsrc + c * 8));
+                    const float4 b1 = __ldg(reinterpret_cast<const float4*>(bsrc + c * 8 + 4));
+                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+                    float y[8];
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        y[i] = __uint_as_float(v[(c & 1) * 8 + i]) + bb[i];
+                        if (p.act == 1) y[i] = fmaxf(y[i], 0.f);
+                        else if (p.act == 2) y[i] = y[i] > 0.f ? y[i] : 0.2f * y[i];
+                        if (p.round_out) y[i] = round_tf32(y[i]);
+                    }
+                    uint32_t h[4], l[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const float a = y[2 * i], b = y[2 * i + 1];
+                        if (p.out16_fmt == 1) {
+                            const __half2 h2 = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
+                            const float2 hf = __half22float2(h2);
+                            const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
+                            h[i] = *reinterpret_cast<const uint32_t*>(&h2);
+                            l[i] = *reinterpret_cast<const uint32_t*>(&l2);
+                        } else {
+                            const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+                            const float2 hf = __bfloat1622float2(h2);
+                            h[i] = *reinterpret_cast<const uint32_t*>(&h2);
+                            l[i] = pack_bf16x2(a - hf.x, b - hf.y);
+                        }
+                    }
+                    const int off = lane * 128 + ((c ^ (lane & 7)) << 4);
+                    *reinterpret_cast<uint4*>(st_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
+                    if (p.out_lo) *reinterpret_cast<uint4*>(st_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
+                }
+                fence_proxy_async_smem();
+                __syncwarp();
+                if (lane == 0 && !(MG_DBGV(p) & 1)) {
+                    tma_store_4d(&tmHi, st_hi, half * 64, ow0, oh0 + quarter * 2, n);
+                    if (p.out_lo) tma_store_4d(&tmLo, st_lo, half * 64, ow0, oh0 + quarter * 2, n);
+                    tma_store_commit();
+                }
+                continue;
+            }
+            // All 64 columns of this warp are read transposed so that every global store request is a full 128-byte line (the
+            // SM->L2 write path is limited by requests, not bytes).  8 lanes serve one pixel: with a 16-bit
+            // output each lane owns 8 consecutive channels (16 B -> 128 B per pixel and request); with an fp32 output it owns
+            // channels q*4..q*4+3 and 32+q*4.. (two requests of 8 x 16 B = 128 B each).
+            {
+                const bool split = p.out != nullptr;                    // fp32 output present -> 4 + 4 channel ownership
+                const int c0 = split ? q * 4 : q * 8, c1 = split ? 32 + q * 4 : q * 8 + 4;
+                const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + half * 64 + c0));
+                const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + half * 64 + c1));
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int r = quarter * 32 + j * 4 + psub;
+                    const int oh = oh0 + (r >> 4), ow = ow0 + (r & 15);
+                    const float4 t0v = *reinterpret_cast<const float4*>(scr + (j * 4 + psub) * kSegAccLd + c0);
+                    const float4 t1v = *reinterpret_cast<const float4*>(scr + (j * 4 + psub) * kSegAccLd + c1);
+                    if (oh >= p.OH || ow >= p.OW || ((MG_DBGV(p) & 1) && t0v.x != 12345.f)) continue;
+                    float y[8] = {t0v.x + b0.x, t0v.y + b0.y, t0v.z + b0.z, t0v.w + b0.w, t1v.x + b1.x, t1v.y + b1.y, t1v.z + b1.z, t1v.w + b1.w};
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        if (p.act == 1) y[i] = fmaxf(y[i], 0.f);
+                        else if (p.act == 2) y[i] = y[i] > 0.f ? y[i] : 0.2f * y[i];
+                        if (p.round_out) y[i] = round_tf32(y[i]);
+                    }
+                    const size_t po = (((size_t)n * p.OH + oh) * p.OW + ow) * 128 + half * 64;
+                    if (p.out) {
+                        *reinterpret_cast<float4*>(p.out + po + c0) = make_float4(y[0], y[1], y[2], y[3]);
+                        *reinterpret_cast<float4*>(p.out + po + c1) = make_float4(y[4], y[5], y[6], y[7]);
+                    }
+                    if (p.out_hi) {
+                        uint32_t h[4], l[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const float a = y[2 * i], b = y[2 * i + 1];
+                            if (p.out16_fmt == 1) {
+                                const __half2 h2 = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
+                                const float2 hf = __half22float2(h2);
+                                const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
+                                h[i] = *reinterpret_cast<const uint32_t*>(&h2);
+                                l[i] = *reinterpret_cast<const uint32_t*>(&l2);
+                            } else {
+                                const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+                                const float2 hf = __bfloat1622float2(h2);
+                                h[i] = *reinterpret_cast<const uint32_t*>(&h2);
+                                l[i] = pack_bf16x2(a - hf.x, b - hf.y);
+                            }
+                        }
+                        uint16_t* ph16 = reinterpret_cast<uint16_t*>(p.out_hi) + po;
+                        uint16_t* pl16 = p.out_lo ? reinterpret_cast<uint16_t*>(p.out_lo) + po : nullptr;
+                        if (!split) {
+                            *reinterpret_cast<uint4*>(ph16 + c0) = make_uint4(h[0], h[1], h[2], h[3]);
+                            if (pl16) *reinterpret_cast<uint4*>(pl16 + c0) = make_uint4(l[0], l[1], l[2], l[3]);
+                        } else {
+                            *reinterpret_cast<uint2*>(ph16 + c0) = make_uint2(h[0], h[1]);
+                            *reinterpret_cast<uint2*>(ph16 + c1) = make_uint2(h[2], h[3]);
+                            if (pl16) {
+                                *reinterpret_cast<uint2*>(pl16 + c0) = make_uint2(l[0], l[1]);
+                                *reinterpret_cast<uint2*>(pl16 + c1) = make_uint2(l[2], l[3]);
+                            }
+                        }
+                    }
+                }
+            }
+        }
+        if (p.tma_store && lane == 0) tma_store_wait_all();
+    } else {
         // ===================== operand builders: thread = pixel row of the tile =====================
-        const int r = threadIdx.x - 32;            // 0..127
+        const int r = threadIdx.x - 256;           // 0..127
         const int tw_l = r & 15, th_l = r >> 4;    // tile = 16 wide x 8 tall
         const int IH = p.OH, IW = p.OW;
         const size_t row_stride = (size_t)IW * p.R * 4, img_stride = (size_t)IH * p.R * row_stride;
@@ -164,170 +283,7 @@ seg_mlp_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             g_seg_prof[3] = (unsigned long long)(clock64() - t_begin); g_seg_prof[4] = (unsigned long long)c_gather;
             g_seg_prof[5] = (unsigned long long)c_wait; g_seg_prof[6] = (unsigned long long)c_store;
         }
-    } else {
-        // ===================== epilogue: 8 warps, (TMEM lane quarter) x (64-column half) =====================
-        const int ew = warp - 5;
-        const int quarter = warp & 3, half = ew >> 2;
-        float* scr = scratch + ew * (32 * 68);
-        const int q = lane & 7, psub = lane >> 3;   // 8 lanes per pixel (32 channels), 4 pixels per pass
-        int it = 0;
-        const bool prof = MG_PROFV(p) && blockIdx.x == 0 && ew == 0 && lane == 0;
-        long long c_wait = 0, c_ld = 0, c_rest = 0, t_begin = prof ? clock64() : 0;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-            const int s = it & 1;
-            const uint32_t ph = (uint32_t)(it >> 1) & 1u;
-            const int n = tile / tiles_per_img, m = tile - n * tiles_per_img;
-            const int oh0 = (m / p.tiles_w) * 8, ow0 = (m % p.tiles_w) * 16;
-            long long t0 = prof ? clock64() : 0;
-            mbar_wait(&t_full[s], ph);
-            if (prof) { const long long t1 = clock64(); c_wait += t1 - t0; t0 = t1; }
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(s * 128 + half * 64);
-            uint32_t v0[16], v1[16], v2[16], v3[16];
-            tmem_ld16(t_row, v0); tmem_ld16(t_row + 16, v1); tmem_ld16(t_row + 32, v2); tmem_ld16(t_row + 48, v3);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(&t_empty[s]);            // accumulator is in registers: release it before the stores
-            if (prof) { const long long t1 = clock64(); c_ld += t1 - t0; t0 = t1; }
-            if (p.tma_store) {
-                // 16-bit outputs only: lane = pixel row of a [32 px][64 ch] box (two image rows of the tile).  Each lane lays its
-                // 128-byte row down in the SWIZZLE_128B pattern (16-byte chunk c at c ^ (row & 7): conflict-free per 8 lanes) and
-                // one lane hands the 4 KB box to the TMA unit, which writes whole lines and clips the part outside the image.
-                uint8_t* st_hi = reinterpret_cast<uint8_t*>(scratch) + ew * 8192;
-                uint8_t* st_lo = st_hi + 4096;
-                if (it > 0) { if (lane == 0) tma_store_wait_read(); __syncwarp(); }
-                const float* bsrc = p.bias + half * 64;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const uint32_t* v = (c >> 1) == 0 ? v0 : (c >> 1) == 1 ? v1 : (c >> 1) == 2 ? v2 : v3;
-                    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bsrc + c * 8));
-                    const float4 b1 = __ldg(reinterpret_cast<const float4*>(bsrc + c * 8 + 4));
-                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                    float y[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        y[i] = __uint_as_float(v[(c & 1) * 8 + i]) + bb[i];
-                        if (p.act == 1) y[i] = fmaxf(y[i], 0.f);
-                        else if (p.act == 2) y[i] = y[i] > 0.f ? y[i] : 0.2f * y[i];
-                        if (p.round_out) y[i] = round_tf32(y[i]);
-                    }
-                    uint32_t h[4], l[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float a = y[2 * i], b = y[2 * i + 1];
-                        if (p.out16_fmt == 1) {
-                            const __half2 h2 = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
-                            const float2 hf = __half22float2(h2);
-                            const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
-                            h[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                            l[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                        } else {
-                            const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                            const float2 hf = __bfloat1622float2(h2);
-                            h[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                            l[i] = pack_bf16x2(a - hf.x, b - hf.y);
-                        }
-                    }
-                    const int off = lane * 128 + ((c ^ (lane & 7)) << 4);
-                    *reinterpret_cast<uint4*>(st_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
-                    if (p.out_lo) *reinterpret_cast<uint4*>(st_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
-                }
-                fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0 && !(MG_DBGV(p) & 1)) {
-                    tma_store_4d(&tmHi, st_hi, half * 64, ow0, oh0 + quarter * 2, n);
-                    if (p.out_lo) tma_store_4d(&tmLo, st_lo, half * 64, ow0, oh0 + quarter * 2, n);
-                    tma_store_commit();
-                }
-                if (prof) c_rest += clock64() - t0;
-                continue;
-            }
-            // All 64 columns of this warp go through the scratch at once so that every global store request is a full
-            // 128-byte line (the SM->L2 write path moves about one request per 11 cycles whatever its size: 32/64-byte
-            // pieces made this kernel store-bound).  8 lanes serve one pixel: with a 16-bit output each lane owns 8
-            // consecutive channels (16 B -> 128 B per pixel and request); with an fp32 output it owns channels
-            // q*4..q*4+3 and 32+q*4.. (two requests of 8 x 16 B = 128 B each).
-            {
-                float4* d = reinterpret_cast<float4*>(scr + lane * 68);
-                if (!(MG_DBGV(p) & 2)) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        d[i] = make_float4(__uint_as_float(v0[4 * i]), __uint_as_float(v0[4 * i + 1]), __uint_as_float(v0[4 * i + 2]), __uint_as_float(v0[4 * i + 3]));
-                        d[4 + i] = make_float4(__uint_as_float(v1[4 * i]), __uint_as_float(v1[4 * i + 1]), __uint_as_float(v1[4 * i + 2]), __uint_as_float(v1[4 * i + 3]));
-                        d[8 + i] = make_float4(__uint_as_float(v2[4 * i]), __uint_as_float(v2[4 * i + 1]), __uint_as_float(v2[4 * i + 2]), __uint_as_float(v2[4 * i + 3]));
-                        d[12 + i] = make_float4(__uint_as_float(v3[4 * i]), __uint_as_float(v3[4 * i + 1]), __uint_as_float(v3[4 * i + 2]), __uint_as_float(v3[4 * i + 3]));
-                    }
-                }
-                __syncwarp();
-                const bool split = p.out != nullptr;                    // fp32 output present -> 4 + 4 channel ownership
-                const int c0 = split ? q * 4 : q * 8, c1 = split ? 32 + q * 4 : q * 8 + 4;
-                const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + half * 64 + c0));
-                const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + half * 64 + c1));
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int r = quarter * 32 + j * 4 + psub;
-                    const int oh = oh0 + (r >> 4), ow = ow0 + (r & 15);
-                    const float4 t0v = *reinterpret_cast<const float4*>(scr + (j * 4 + psub) * 68 + c0);
-                    const float4 t1v = *reinterpret_cast<const float4*>(scr + (j * 4 + psub) * 68 + c1);
-                    if (oh >= p.OH || ow >= p.OW || ((MG_DBGV(p) & 1) && t0v.x != 12345.f)) continue;
-                    float y[8] = {t0v.x + b0.x, t0v.y + b0.y, t0v.z + b0.z, t0v.w + b0.w, t1v.x + b1.x, t1v.y + b1.y, t1v.z + b1.z, t1v.w + b1.w};
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        if (p.act == 1) y[i] = fmaxf(y[i], 0.f);
-                        else if (p.act == 2) y[i] = y[i] > 0.f ? y[i] : 0.2f * y[i];
-                        if (p.round_out) y[i] = round_tf32(y[i]);
-                    }
-                    const size_t po = (((size_t)n * p.OH + oh) * p.OW + ow) * 128 + half * 64;
-                    if (p.out) {
-                        *reinterpret_cast<float4*>(p.out + po + c0) = make_float4(y[0], y[1], y[2], y[3]);
-                        *reinterpret_cast<float4*>(p.out + po + c1) = make_float4(y[4], y[5], y[6], y[7]);
-                    }
-                    if (p.out_hi) {
-                        uint32_t h[4], l[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float a = y[2 * i], b = y[2 * i + 1];
-                            if (p.out16_fmt == 1) {
-                                const __half2 h2 = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
-                                const float2 hf = __half22float2(h2);
-                                const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
-                                h[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                                l[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                            } else {
-                                const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                                const float2 hf = __bfloat1622float2(h2);
-                                h[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                                l[i] = pack_bf16x2(a - hf.x, b - hf.y);
-                            }
-                        }
-                        uint16_t* ph16 = reinterpret_cast<uint16_t*>(p.out_hi) + po;
-                        uint16_t* pl16 = p.out_lo ? reinterpret_cast<uint16_t*>(p.out_lo) + po : nullptr;
-                        if (!split) {
-                            *reinterpret_cast<uint4*>(ph16 + c0) = make_uint4(h[0], h[1], h[2], h[3]);
-                            if (pl16) *reinterpret_cast<uint4*>(pl16 + c0) = make_uint4(l[0], l[1], l[2], l[3]);
-                        } else {
-                            *reinterpret_cast<uint2*>(ph16 + c0) = make_uint2(h[0], h[1]);
-                            *reinterpret_cast<uint2*>(ph16 + c1) = make_uint2(h[2], h[3]);
-                            if (pl16) {
-                                *reinterpret_cast<uint2*>(pl16 + c0) = make_uint2(l[0], l[1]);
-                                *reinterpret_cast<uint2*>(pl16 + c1) = make_uint2(l[2], l[3]);
-                            }
-                        }
-                    }
-                }
-                __syncwarp();
-            }
-            if (prof) c_rest += clock64() - t0;
-        }
-        if (p.tma_store && lane == 0) tma_store_wait_all();
-        if (prof) {
-            g_seg_prof[7] = (unsigned long long)(clock64() - t_begin); g_seg_prof[8] = (unsigned long long)c_wait;
-            g_seg_prof[9] = (unsigned long long)c_ld; g_seg_prof[10] = (unsigned long long)c_rest;
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) { tc_fence_after(); tmem_dealloc(tmem_base, 256); }
 }
 
 // w [128][Cin<=4][3][3] fp32 -> bf16 [128][128]: k = part*36 + tap*4 + ci, parts (W_hi, W_hi, W_lo), zero tail.
@@ -349,8 +305,7 @@ __global__ void pack_weight_seg_tc_kernel(const float* __restrict__ w, __nv_bflo
 
 using namespace mg;
 
-// Debug: [0] MMA thread total, [1] wait accumulator-empty, [2] wait operand-full; [3] builder total, [4] gather, [5] wait
-// operand-empty, [6] store+fence; [7] epilogue warp 0 total, [8] wait accumulator-full, [9] TMEM load, [10] transpose+stores.
+// Debug: [3] builder total, [4] gather, [5] wait operand-empty, [6] store+fence (CTA 0, probe build with MG_DBG & 16).
 extern "C" int mg_debug_seg_prof(unsigned long long* host16) {
     if (!host16) return set_error(-1, "mg_debug_seg_prof: null pointer");
     cudaError_t e = cudaDeviceSynchronize();
@@ -381,7 +336,6 @@ extern "C" int mg_conv_seg_tc(const mg_thin_args* a, void* stream_) {
     p.round_out = a->round_out; p.act = a->act;
     p.N = a->N; p.OH = a->OH; p.OW = a->OW; p.R = a->seg_resize > 0 ? a->seg_resize : 1;
     p.tiles_w = (a->OW + 15) / 16; p.tiles_h = (a->OH + 7) / 8; p.num_tiles = p.tiles_w * p.tiles_h * a->N;
-    p.idesc = umma_idesc_16(128, 128, 2);
 #ifdef MG_PROBES
     p.prof = probe_bits() & 16;
     p.dbg = probe_bits() & 3;
@@ -408,7 +362,7 @@ extern "C" int mg_conv_seg_tc(const mg_thin_args* a, void* stream_) {
         if (!rc && a->out_lo) rc = encode_tensor_map(&tmLo, a->out_lo, dt, 4, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
-    const size_t smem_bytes = 1024 + 3 * kSegTileBytes + 1024 + 8 * 32 * 68 * 4;
+    const size_t smem_bytes = 1024 + 3 * kSegTileBytes + 1024 + 128 * kSegAccLd * 4;
     static thread_local int attr_dev = -1;
     int dev = 0; cudaGetDevice(&dev);
     if (attr_dev != dev) {

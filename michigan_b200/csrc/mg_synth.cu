@@ -6,7 +6,7 @@
 //   * the orientation RGB map of --use_ig: [(cos 2t + 1)/2, (sin 2t + 1)/2, 0.5] * mask, quantised to uint8 by
 //     PIL and back to [0,1] by ToTensor (base_dataset.py:363-385 trans_orient_to_rgb);
 //   * the random disk "hole" inside the hair mask (base_dataset.py:335-361 generate_hole).
-// At B200 speeds (2000+ images/s on 8 GPUs) a CPU loader cannot produce these fast enough; the kernels below produce them for
+// At multi-GPU training speeds a CPU loader cannot produce these fast enough; the kernels below produce them for
 // a whole batch from device-resident label / orientation maps.  Random draws are INPUTS (Gaussian fields, uniforms), so the
 // arithmetic is testable against the reference functions on identical draws.
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Drop the B200 operator classes into an (unmodified) MichiGAN checkout.
+"""Drop the sm_90a operator classes into an (unmodified) MichiGAN checkout.
 
 The reference resolves networks by *name* at run time: `find_class_in_module(name + 'generator',
 'models.networks.generator')` scans the module's __dict__ (util/util.py:180-192,

@@ -1,4 +1,4 @@
-"""Launcher: run an UNMODIFIED MichiGAN script (train.py / inference.py) on the B200 kernels, one process per GPU.
+"""Launcher: run an UNMODIFIED MichiGAN script (train.py / inference.py) on the sm_90a kernels, one process per GPU.
 
     python -m michigan_b200.launch <reference_root> inference.py --name MichiGAN --netG spadeb ...          # 1 GPU
     torchrun --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 -m michigan_b200.launch <reference_root> train.py \\

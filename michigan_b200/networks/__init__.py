@@ -1,6 +1,6 @@
 """Operator layer of the hot path — the classes the reference looks up by name in
 `models.networks.{generator,discriminator,normalization,architecture,encoder,sync_batchnorm}`
-(models/networks/__init__.py:16-85), re-implemented on hand-written sm_100a kernels."""
+(models/networks/__init__.py:16-85), re-implemented on hand-written sm_90a kernels."""
 import torch
 
 from .base_network import BaseNetwork

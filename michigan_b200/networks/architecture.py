@@ -1,13 +1,13 @@
 """SPADEResnetBlock — constructor, attribute names and state-dict keys of the reference's
-models/networks/architecture.py:23-85; forward = fused sm_100a kernels.
+models/networks/architecture.py:23-85; forward = fused sm_90a kernels.
 
 Per block (x at 1/2^x_shift of the block's resolution; the nn.Upsample of generator.py:72 is folded
 into the consumers' loads):
 
     stats(x)                                    one HBM pass, shared by norm_0 and norm_s
     actv_k  = relu(conv3x3(seg'))               thin direct conv, seg read through nearest resize
-    h_k     = act(x_hat*(1+gamma)+beta)         tcgen05 implicit GEMM (K=9*128, N=2C) + SPADE epilogue
-    conv_0 / conv_1 / conv_s                    tcgen05 implicit GEMM + bias / residual / blend epilogue
+    h_k     = act(x_hat*(1+gamma)+beta)         wgmma implicit GEMM (K=9*128, N=2C) + SPADE epilogue
+    conv_0 / conv_1 / conv_s                    wgmma implicit GEMM + bias / residual / blend epilogue
 """
 from types import SimpleNamespace
 

@@ -4,7 +4,7 @@
 additionally keep the fp32 value of every tensor the gradient GEMMs need (read as TF32 by the wgrad / dgrad kernels);
 backward = explicit reverse pass over the saved per-block state:
 
-    conv  : dW = mg_conv_wgrad (tcgen05, MN-major, split-K);  dX = mg_conv_igemm on dY with flipped sub-kernels
+    conv  : dW = mg_conv_wgrad (mma.sync, MN-major, split-K);  dX = mg_conv_igemm on dY with flipped sub-kernels
     SPADE : mg_spade_bwd (dgamma|dbeta operand, dxhat, BN sums)  ->  gamma/beta GEMM wgrad + dgrad  ->  thin wgrad
     BN/IN : mg_bn_bwd_apply / mg_in_bwd (statistics all-reduced across ranks like the forward ones)
     SN    : mg_spectral_norm_bwd (u, v constants, as torch's spectral_norm autograd)

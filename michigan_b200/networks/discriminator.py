@@ -1,9 +1,9 @@
 """MultiscaleDiscriminator / NLayerDiscriminator — constructors, option hooks, forward signature and
 state-dict layout of the reference's models/networks/discriminator.py:14-120 (norm_D =
-'spectralinstance'); forward on the sm_100a kernels:
+'spectralinstance'); forward on the sm_90a kernels:
 
     model0      7->64 k4 s2 p2 + bias + LeakyReLU           thin direct conv (channels padded to 8)
-    model1..3   SN conv k4 (s2,s2,s1) p2, no bias           tcgen05 implicit GEMM (stride via TMA elementStrides)
+    model1..3   SN conv k4 (s2,s2,s1) p2, no bias           wgmma implicit GEMM (stride via TMA elementStrides)
                 InstanceNorm2d(affine=False) + LeakyReLU     per-(n,c) stats pass + normalise pass
     model4      512->1 k4 s1 p2 + bias                       warp-per-pixel dot product
     downsample  avg_pool2d(3, 2, 1, count_include_pad=False) on the 8-channel NHWC input

@@ -1,5 +1,5 @@
 """SPADEBGenerator (`--netG spadeb`) — constructor, forward signature and state-dict layout of the
-reference's models/networks/generator.py:19-230; the forward runs on the sm_100a kernels.
+reference's models/networks/generator.py:19-230; the forward runs on the sm_90a kernels.
 
 Data layout: every internal activation is NHWC fp32 in HBM; tensors that feed a tensor-core conv are
 written TF32-rounded by their producer; the 2x nearest upsamples (generator.py:72,163-210) and the
@@ -17,9 +17,8 @@ from .base_network import BaseNetwork
 from .encoder import BackgroundEncode2, ImageEncoder3
 from .prep import PackCache, SpectralNormBatch
 
-# MICHIGAN_B200_OVERLAP=1: background encoder on a second stream.  Measured same-box (profiles/r02_ab_overlap.log): 23.04 vs 22.99 ms
-# per forward, i.e. nothing - the low-resolution blocks are short and the encoder's 148-CTA kernels cannot share an SM with a
-# 227 KB-smem GEMM CTA anyway - so it stays off.
+# MICHIGAN_B200_OVERLAP=1: background encoder on a second stream (off by default: the low-resolution blocks are short and the
+# encoder's one-CTA-per-SM kernels cannot share an SM with a large-smem GEMM CTA anyway).
 _OVERLAP = os.environ.get("MICHIGAN_B200_OVERLAP", "0") == "1"
 
 
@@ -126,7 +125,7 @@ class SPADEBGenerator(BaseNetwork):
         ins_tag = input_tag[:, 1:2]
         sv = (lambda: SimpleNamespace()) if save is not None else (lambda: None)
         Sfc, Sbg = sv(), sv()
-        # The background encoder (generator.py:144-147; full-resolution maps, 148-CTA kernels) is independent of the reference
+        # The background encoder (generator.py:144-147; full-resolution maps, one-CTA-per-SM kernels) is independent of the reference
         # encoder and of head_0 / G_middle_0 / G_middle_1, whose 8x8..32x32 maps give the persistent GEMM kernels only 16..128 tiles:
         # it runs on a second stream and fills the SMs those kernels leave idle; the main stream joins before up_0's blend.
         overlap = _OVERLAP and input_tag.is_cuda

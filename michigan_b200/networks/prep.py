@@ -1,4 +1,4 @@
-"""Per-forward weight preparation: batched spectral norm + operand packing for the tcgen05 kernels.
+"""Per-forward weight preparation: batched spectral norm + operand packing for the tensor-core kernels.
 
 State-dict tensors stay OIHW fp32 with the reference's key layout (`weight_orig/_u/_v`, SURVEY.md §5);
 the packed copies (tap-major K, W/sigma applied, TF32-rounded) are transient device buffers that are

@@ -2,7 +2,7 @@
 
 The reference's data-parallel runtime is single-process torch.nn.DataParallel plus a Python
 thread/queue master-slave SyncBN (batchnorm.py:51-145, comm.py:18-137, replicate.py:27-94).  The
-B200 design is one process per GPU:
+The design is one process per GPU:
 
   * SyncBN statistics: every rank pushes its [sum | sum of squares | sample count] vector into all
     peers' symmetric buffers over NVLink and sums the world_size vectors in rank order inside ONE

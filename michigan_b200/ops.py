@@ -1,7 +1,7 @@
 """Functional wrappers: torch CUDA tensors in, C-ABI calls on the current stream, torch tensors out.
 
 PyTorch is plumbing here (device memory, streams); every arithmetic op below runs in
-libmichigan_sm100.so.  Activations are NHWC fp32 ([N,H,W,C] contiguous).
+libmichigan_sm90.so.  Activations are NHWC fp32 ([N,H,W,C] contiguous).
 """
 import ctypes as C
 import math
@@ -56,16 +56,16 @@ def _chk(t, name, dtype=torch.float32):
         raise ValueError("%s must be contiguous" % name)
 
 
-_SPADE_BN_MAX = int(os.environ.get("MG_SPADE_BN", "256"))
-# N tile of split-precision 3x3 / stride-1 convs routed to the M-tile-group kernel (0 = the launcher's default: min(Cout, 256)).
-# 64: merged accumulators of 128 columns for every such layer (double-buffered groups; weights re-read per 256 instead of 128 pixels)
+# widest GEMM N tile of the implicit-GEMM kernels (128 accumulator columns per consumer warpgroup)
+_SPADE_BN_MAX = 128
+# N tile of split-precision 3x3 / stride-1 convs routed to the M-tile-group kernel (0 = the launcher's default: min(Cout, 128)).
+# 64: merged accumulators of 128 columns for every such layer
 _CONV3_BN = int(os.environ.get("MG_CONV3_BN", "0"))
 
 
 def spade_bn(c):
     """GEMM N tile used for a gamma|beta operand of `c` channels (must match the weight packing: [gamma(BN/2) | beta(BN/2)] per
-    N tile).  MG_SPADE_BN=128: 128-column tiles, which the 3x3 M-tile-group kernel can double buffer (two M tiles share every
-    weight slot: half the weight bytes through L2 per pixel, at the price of N = 128 MMAs)."""
+    N tile)."""
     return _SPADE_BN_MAX if 2 * c >= _SPADE_BN_MAX else max(64, 2 * c)
 
 
@@ -119,7 +119,7 @@ def pack_weight_thin(w_oihw, cin_pad):
 def conv_igemm(x, wpack, cout, kh, kw, stride=1, pad=0, *, act=ACT_NONE, round_out=False, bias=None, res=None,
                res_shift=0, pscale=None, pmul=None, blend=None, spade=None, bn=0, max_ctas=0, out=None, out_hw=None, _extra=None,
                a_fmt=TF32, x_lo=None, out16=None, want_f32=True, aux=None):
-    """Implicit-GEMM conv on tcgen05.  x: [N,H,W,Cin]; returns [N,OH,OW,cout].
+    """Implicit-GEMM conv on wgmma.  x: [N,H,W,Cin]; returns [N,OH,OW,cout].
 
     blend = (bf[N,OH,OW,cout], hair[N,MH,MW], back[N,MH,MW], mask_stride)
     spade = (xsrc[N,OH>>s,OW>>s,cout], x_shift, nscale[c], nshift[c], gbias1[c], bbias[c])
@@ -474,7 +474,7 @@ def avgpool3s2(x):
 
 # ------------------------------------------------------------------------------------------ backward
 def conv_wgrad(dy, x, kh, kw, stride=1, pad=0):
-    """Packed weight gradient [Cout][kh*kw*Cin] of an implicit-GEMM conv (tcgen05, split-K)."""
+    """Packed weight gradient [Cout][kh*kw*Cin] of an implicit-GEMM conv (tensor cores, split-K)."""
     _chk(dy, "dy"); _chk(x, "x")
     N, H, W, Cin = x.shape
     _, OH, OW, Cout = dy.shape
@@ -493,7 +493,7 @@ def dgrad_geometry(k, stride, pad, r):
 
 
 def conv_dgrad(dy, w_oihw, in_hw, stride=1, pad=0, inv_sigma=None, out=None, accumulate=False, dy16=None):
-    """dX [N,H,W,Cin] of y = conv(x, w, stride, pad) given dY [N,OH,OW,Cout]; tcgen05 implicit GEMM on dY
+    """dX [N,H,W,Cin] of y = conv(x, w, stride, pad) given dY [N,OH,OW,Cout]; wgmma implicit GEMM on dY
     with flipped/transposed (sub-)kernels, one launch per output parity class (stride^2).
     dy16: bf16 copy of dY -> the GEMM runs with bf16 operands (weights converted after packing), fp32 accumulation."""
     _chk(dy, "dy"); _chk(w_oihw, "w"); _chk(dy16, "dy16", torch.bfloat16)

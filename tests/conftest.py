@@ -13,7 +13,7 @@ def pytest_configure(config):
     import torch
     # the CPU oracle scales poorly past ~32 threads on the many-core GPU hosts
     torch.set_num_threads(min(32, os.cpu_count() or 1))
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,6 +1,5 @@
 """Multi-GPU parity (NCCL, one process per GPU): runs tests/nccl_worker.py under torch.distributed.run on 2 GPUs and
-asserts its report.  Skipped on a single-GPU box (the driver's `pytest -m gpu` tier runs on one GPU; `tools/gpu_multi.sh`
-and gpurun --gpus 2 run it for real)."""
+asserts its report.  Skipped on a single-GPU machine."""
 import json
 import os
 import socket

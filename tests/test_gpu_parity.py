@@ -282,7 +282,7 @@ def test_backward_chain_smooth_loss_vs_oracle():
     ~5e-4), and LeakyReLU / ReLU derivatives jump at 0, so ~0.05 % of the activation-derivative masks differ
     from the fp32 oracle per layer: measured ~2e-2 per discriminator layer, ~1e-2 per SPADE block, compounding
     to ~0.12 at the reference encoder (7 blocks upstream); single-block and single-kernel gradients are checked
-    to 1e-2 / 5e-5 by tools/debug_bwd.py and tools/probe_kernels.py bwd2 (profiles/).  Tensors whose reference
+    to 1e-2 / 5e-5 by tools/debug_bwd.py and tools/probe_kernels.py bwd2.  Tensors whose reference
     norm is below 1e-4 (1e-2 for 1-D sums) of the largest are measured against that floor."""
     from michigan_b200 import networks
     from michigan_b200.options import make_opt

@@ -79,7 +79,7 @@ def group_igemm2():
     igemm_case(2, 66, 66, 64, 64, 4, 2, 1, bias=True, act=1 if False else 0)  # k4 s2 p1 (bg encoder after pad)
     igemm_case(2, 64, 64, 64, 128, 3, 2, 1)       # partial-conv geometry
     igemm_case(2, 32, 32, 64, 64, 3, 1, 1, exact=False, tol=3e-3, name="igemm unrounded inputs (tf32 hw rounding)")
-    # larger: multiple tiles per CTA (persistence + both TMEM buffers + ring wrap)
+    # larger: multiple tiles per CTA (persistence + ring wrap)
     igemm_case(4, 128, 128, 128, 256, 3, 1, 1)
 
 
@@ -301,7 +301,7 @@ def group_halo(pw="16", bo="1"):
     igemm_case(2, 32, 32, 128, 256, 3, 1, 1)
     igemm_case(1, 64, 40, 64, 128, 3, 1, 1, bn=64)       # ragged width (40 = 5 tiles of 8), two N tiles
     igemm_case(2, 24, 20, 64, 64, 3, 1, 1)               # partial tiles in both directions
-    igemm_case(4, 128, 128, 128, 256, 3, 1, 1)           # many tiles per CTA: ring wrap, both TMEM buffers
+    igemm_case(4, 128, 128, 128, 256, 3, 1, 1)           # many tiles per CTA: ring wrap
     g = torch.Generator(device="cpu").manual_seed(21)
     for (N, h, Cin, Cout) in ((2, 32, 64, 64), (1, 64, 256, 128), (2, 48, 128, 256)):
         x = torch.randn(N, Cin, h, h, generator=g).to(dev)
@@ -415,7 +415,7 @@ def group_segtc():
 
 
 def group_bwd():
-    """tcgen05 weight gradient (MN-major operands, split-K) and data gradient (transposed conv)."""
+    """Tensor-core weight gradient (MN-major operands, split-K) and data gradient (transposed conv)."""
     g = torch.Generator(device="cpu").manual_seed(31)
     for (N, h, Cin, Cout, k, s_, p_) in ((2, 32, 64, 64, 3, 1, 1), (2, 32, 128, 256, 3, 1, 1), (2, 33, 64, 128, 4, 2, 2),
                                          (2, 65, 64, 128, 4, 1, 2), (2, 34, 64, 64, 4, 2, 0), (2, 32, 64, 128, 3, 2, 1),

@@ -1,5 +1,5 @@
 """Launch ONE kernel of the hot path a few times at its benchmark shape (N = 8, 512x512) - the target of `ncu --set full`
-(tools/ncu_kernels.sh).  argv[1]: spade | group | wgrad16 | wgrad32 | seg | stats | spade_bwd | dconv"""
+or of a profiler.  argv[1]: spade | group | wgrad16 | wgrad32 | seg | stats | spade_bwd | dconv"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -43,7 +43,7 @@ else:
 for _ in range(4):
     f()
 torch.cuda.synchronize()
-if os.environ.get("MG_TIME"):          # not under ncu: average of 20 launches, CUDA events
+if os.environ.get("MG_TIME"):          # not under a profiler: average of 20 launches, CUDA events
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(20):
