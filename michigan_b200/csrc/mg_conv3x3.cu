@@ -12,10 +12,13 @@
 // Same operand formats (TF32 / fp16 / bf16, split precision merged or 3-pass), same epilogues (mg_epilogue.cuh), same
 // results as mg_igemm.cu up to accumulation order.
 //
-// Warp roles (288 threads): warps 0..7 wgmma consumers (rows 0-63 / 64-127 of both M tiles) + epilogue, warp 8 TMA producer.
+// Warp roles (384 threads): warps 0..7 wgmma consumers (rows 0-63 / 64-127 of both M tiles) + epilogue, 232 registers each;
+// warps 8..11 the producer warpgroup, 40 registers, one thread of which issues the TMA loads.  The mainloop keeps one wgmma
+// group in flight (see igemm_tf32_kernel).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstring>
+#include <type_traits>
 #include "mg_ptx.cuh"
 #include "mg_internal.h"
 #include "mg_epilogue.cuh"
@@ -39,10 +42,12 @@ struct Conv3Params {
 //   plain          : 9 (tap)                                   MMA N = BN
 //   merged split   : hi 9 x [W_hi;W_lo] (N = 2BN), lo 9 x W_hi (N = BN)
 //   3-pass split   : hi 18 = tap x {W_hi, W_lo} (N = BN),   lo 9 x W_hi (N = BN)
-template <int SPEC, int CW>
+// FMT, BN, MERGED: compile-time wgmma shape and type; SPEC, CW: epilogue specialisation (as igemm_tf32_kernel).
+template <int FMT, int BN, bool MERGED, int SPEC, int CW>
 __global__ void __launch_bounds__(kThreads, 1)
 conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                      const __grid_constant__ CUtensorMap tmB, const Conv3Params q) {
+    constexpr int kAcc = MERGED ? 2 * BN : BN;   // accumulator columns
     const IgemmParams& p = q.g;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -70,9 +75,11 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     const int groups_per_img = q.groups_w * p.tiles_h;
     const bool split = p.parts > 1;
 
-    if (warp == kNumEpiWarps) {
+    if (warp >= kNumEpiWarps) {
         // ===================== TMA producer (one thread): A patches are issued one item ahead of the weight stream ===========
-        if (lane == 0) {
+        // The producer warpgroup hands its registers to the consumers; one thread of it issues every TMA load.
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == kNumEpiWarps && lane == 0) {
             int bs = 0, as_ = 0;
             uint32_t bph = 0, aphs = 0;
             // A-patch cursor: runs up to kASlots - 1 items ahead of the weight stream (the next patch is requested as soon as
@@ -82,7 +89,7 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             auto issue_a = [&](bool must) -> bool {
                 if (gia >= q.num_groups) return false;
                 if (!must && !mbar_test_wait(&aempty[as_], aphs ^ 1)) return false;
-                if (must) mbar_wait(&aempty[as_], aphs ^ 1);
+                if (must) mbar_wait_report(&aempty[as_], aphs ^ 1);
                 const int mga = gia / p.n_tiles;
                 const int gwa = mga % q.groups_w, tha = (mga / q.groups_w) % p.tiles_h, tna = mga / groups_per_img;
                 const int kca = split ? (ita >> 1) : ita, parta = split ? (ita & 1) : 0;
@@ -106,7 +113,7 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                         int tap, wsel;
                         if (steps == 18) { tap = st >> 1; wsel = st & 1; } else { tap = st; wsel = 0; }
                         const int kofs = (split ? (tap * 2 + wsel) : tap) * p.Cin + kc * p.kelem;
-                        mbar_wait(&bempty[bs], bph ^ 1);
+                        mbar_wait_report(&bempty[bs], bph ^ 1);
                         uint8_t* sb = b_ring + (size_t)bs * q.b_slot_bytes;
                         if (p.merged && part == 0) {
                             mbar_arrive_expect_tx(&bfull[bs], (uint32_t)(2 * p.BN * 128));
@@ -124,61 +131,103 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     } else {
         // ===================== consumers: warpgroup wg multiplies rows 64*wg.. of BOTH M tiles of a group, then all 8 warps
         // run the epilogue of M tile 0 and of M tile 1
+        setmaxnreg_inc<kConsumerRegs>();
         const int wg = warp >> 2;
         const int quarter = warp & 3;
         const int half = warp >> 2;
         float* scr = reinterpret_cast<float*>(smem + p.epi_off) + warp * (32 * (CW + 4));
         const uint32_t a_base0 = smem_u32(a_ring), b_base0 = smem_u32(b_ring);
-        float acc0[64], acc1[64];
+        float acc0[kAcc / 2], acc1[kAcc / 2];
         int bs = 0, as_ = 0;
         uint32_t bph = 0, aphs = 0;
+        // Pipelined mainloop: one wgmma group stays in flight.  After a step commits, wait_group 1 retires the step before
+        // it, and only then is that step's weight slot released; a patch is released by the wait that retires its last step
+        // (the first step of the next item).  held_*: slots whose release waits for that retirement.
+        int held_b = -1, held_a = -1;
+        auto release_held = [&]() {
+            __syncwarp();
+            if (lane == 0) {   // this warp's reads of the slots are done
+                if (held_b >= 0) mbar_arrive(&bempty[held_b]);
+                if (held_a >= 0) mbar_arrive(&aempty[held_a]);
+            }
+            held_b = held_a = -1;
+        };
         for (int gi = blockIdx.x; gi < q.num_groups; gi += gridDim.x) {
             const int nt = gi % p.n_tiles;
             const int mg = gi / p.n_tiles;
             const int gw = mg % q.groups_w, th = (mg / q.groups_w) % p.tiles_h, tn = mg / groups_per_img;
             for (int it = 0; it < q.n_items; ++it) {
                 const int part = split ? (it & 1) : 0;
-                const int n = (p.merged && part == 1) ? p.BN : p.acc_cols;
                 mbar_wait(&afull[as_], aphs);
                 // rows 64.. of an M tile are its pixel rows 8.., eight patch rows further on
                 const uint32_t a_base = a_base0 + (uint32_t)(as_ * kPatchBytes) + (uint32_t)(wg * 8 * kPatchW * 128);
                 const int steps = part ? q.steps_lo : q.steps_hi;
-                for (int st = 0; st < steps; ++st) {
-                    const int tap = steps == 18 ? (st >> 1) : st;
-                    const int kh = tap / 3, kw = tap - kh * 3;
-                    mbar_wait(&bfull[bs], bph);
-                    // tap (kh, kw) of M tile mt = the patch read from row kh*18 + kw + 8*mt on; 8-pixel row groups are 18 rows apart
-                    const uint32_t a_tap = a_base + (uint32_t)((kh * kPatchW + kw) * 128);
-                    const uint64_t db = wg_desc_sw128(b_base0 + (uint32_t)(bs * q.b_slot_bytes), 1024);
-                    wgmma_fence();
+                // the steps of one item at MMA width N, both M tiles
+                auto item = [&](auto n_cols) {
+                    constexpr int N = decltype(n_cols)::value;
+                    for (int st = 0; st < steps; ++st) {
+                        const int tap = steps == 18 ? (st >> 1) : st;
+                        const int kh = tap / 3, kw = tap - kh * 3;
+                        mbar_wait(&bfull[bs], bph);
+                        // tap (kh, kw) of M tile mt = the patch read from row kh*18 + kw + 8*mt on; 8-pixel row groups are 18 rows apart
+                        const uint32_t a_tap = a_base + (uint32_t)((kh * kPatchW + kw) * 128);
+                        const uint64_t db = wg_desc_sw128(b_base0 + (uint32_t)(bs * q.b_slot_bytes), 1024);
+                        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint32_t accum = (it | st | k) != 0 ? 1u : 0u;
-                        const uint64_t da0 = wg_desc_sw128(a_tap + (uint32_t)(k * 32), (uint32_t)(kPatchW * 128));
-                        const uint64_t da1 = wg_desc_sw128(a_tap + (uint32_t)(8 * 128 + k * 32), (uint32_t)(kPatchW * 128));
-                        wgmma_k32b(acc0, n, p.a_fmt, da0, db + (uint64_t)(2 * k), accum);
-                        wgmma_k32b(acc1, n, p.a_fmt, da1, db + (uint64_t)(2 * k), accum);
+                        for (int k = 0; k < 4; ++k) {
+                            const uint32_t accum = (it | st | k) != 0 ? 1u : 0u;
+                            const uint64_t da0 = wg_desc_sw128(a_tap + (uint32_t)(k * 32), (uint32_t)(kPatchW * 128));
+                            const uint64_t da1 = wg_desc_sw128(a_tap + (uint32_t)(8 * 128 + k * 32), (uint32_t)(kPatchW * 128));
+                            wgmma_step<FMT, N>(acc0, da0, db + (uint64_t)(2 * k), accum);
+                            wgmma_step<FMT, N>(acc1, da1, db + (uint64_t)(2 * k), accum);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        release_held();
+                        held_b = bs;
+                        if (++bs == q.b_slots) { bs = 0; bph ^= 1; }
                     }
-                    wgmma_commit();
-                    wgmma_wait_all();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&bempty[bs]);     // this warp's reads of the slot are done
-                    if (++bs == q.b_slots) { bs = 0; bph ^= 1; }
-                }
-                if (lane == 0) mbar_arrive(&aempty[as_]);
+                };
+                // merged split precision: hi items are A_hi x [W_hi ; W_lo] (N = 2*BN), lo items A_lo x W_hi (N = BN)
+                if (MERGED && part == 1) item(std::integral_constant<int, BN>{});
+                else item(std::integral_constant<int, kAcc>{});
+                held_a = as_;
                 if (++as_ == kASlots) { as_ = 0; aphs ^= 1; }
             }
+            wgmma_wait<0>();
+            wgmma_fence_operand(acc0);
+            wgmma_fence_operand(acc1);
+            release_held();
             bar_sync(1, kNumEpiWarps * 32);
-            acc_store(acc_tile, p.acc_ld, acc0, p.acc_cols, wg * 64);
+            acc_store(acc_tile, p.acc_ld, acc0, kAcc, wg * 64);
             bar_sync(1, kNumEpiWarps * 32);
             epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM, th, tn, quarter, half, lane);
             bar_sync(1, kNumEpiWarps * 32);
-            acc_store(acc_tile, p.acc_ld, acc1, p.acc_cols, wg * 64);
+            acc_store(acc_tile, p.acc_ld, acc1, kAcc, wg * 64);
             bar_sync(1, kNumEpiWarps * 32);
             epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM + 1, th, tn, quarter, half, lane);
         }
     }
 }
+
+struct Conv3Launch {
+    const CUtensorMap *tmA, *tmA2, *tmB;
+    const Conv3Params* q;
+    int grid;
+    size_t smem_bytes;
+    cudaStream_t stream;
+    template <int FMT, int BN, bool MERGED, int SPEC, int CW>
+    int run() const {
+        if constexpr (conv_variant_exists<FMT, BN, MERGED, SPEC, CW>()) {
+            static thread_local int attr_dev = -1;
+            return launch_conv_kernel(conv3x3_group_kernel<FMT, BN, MERGED, SPEC, CW>, attr_dev, grid, smem_bytes, stream, *tmA, *tmA2,
+                                      *tmB, *q);
+        } else {
+            return set_error(-14, "conv3x3: no kernel variant for format %d, BN %d, merged %d, SPEC %d, CW %d", FMT, BN, (int)MERGED,
+                             SPEC, CW);
+        }
+    }
+};
 
 // Returns 1 when the launch was taken by this kernel, 0 when the shape is not eligible (caller uses mg_igemm.cu's path),
 // < 0 / > 0 on error.
@@ -244,31 +293,12 @@ int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw,
         if (rc) return rc;
     }
     const size_t smem_bytes = ring_bytes + 1024 + 512 + scratch_bytes + acc_bytes;
-    static thread_local int attr_set_dev = -1;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (attr_set_dev != dev) {
-        cudaError_t e = cudaSuccess;
-        const void* kernels[6] = {(const void*)conv3x3_group_kernel<0, 16>, (const void*)conv3x3_group_kernel<0, 32>,
-                                  (const void*)conv3x3_group_kernel<1, 16>, (const void*)conv3x3_group_kernel<1, 32>,
-                                  (const void*)conv3x3_group_kernel<2, 16>, (const void*)conv3x3_group_kernel<2, 32>};
-        for (int i = 0; i < 6 && e == cudaSuccess; ++i)
-            e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        attr_set_dev = dev;
-    }
     int grid = num_sms();
     if (a->max_ctas > 0 && a->max_ctas < grid) grid = a->max_ctas;
     if (grid > q.num_groups) grid = q.num_groups;
-#define MG_LAUNCH3(S, C) conv3x3_group_kernel<S, C><<<grid, kThreads, smem_bytes, stream>>>(tmA, tmA2, tmB, q)
-    if (spec == 1) { if (cw == 32) MG_LAUNCH3(1, 32); else MG_LAUNCH3(1, 16); }
-    else if (spec == 2) { if (cw == 32) MG_LAUNCH3(2, 32); else MG_LAUNCH3(2, 16); }
-    else { if (cw == 32) MG_LAUNCH3(0, 32); else MG_LAUNCH3(0, 16); }
-#undef MG_LAUNCH3
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error((int)e, "conv3x3 launch: %s", cudaGetErrorString(e));
-    return 1;
+    const Conv3Launch l{&tmA, &tmA2, &tmB, &q, grid, smem_bytes, stream};
+    const int rc = dispatch_conv_variant(l, p.a_fmt, BN, p.merged != 0, spec, cw);
+    return rc == 0 ? 1 : rc;
 }
 
 }  // namespace mg

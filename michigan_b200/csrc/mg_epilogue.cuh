@@ -12,8 +12,13 @@
 namespace mg {
 
 constexpr int kNumEpiWarps = 8;
-// warps 0..7: two consumer warpgroups (wgmma on rows 0-63 / 64-127 of the 128-pixel tile, then the epilogue), warp 8: TMA producer
-constexpr int kThreads = kNumEpiWarps * 32 + 32;  // 288
+// warps 0..7: two consumer warpgroups (wgmma on rows 0-63 / 64-127 of the 128-pixel tile, then the epilogue);
+// warps 8..11: the producer warpgroup, in which one thread issues the TMA loads.  A whole warpgroup for the producer lets it
+// hand registers back with setmaxnreg: 40 x 128 + 232 x 256 = 64,512 of the SM's 65,536.
+constexpr int kThreads = kNumEpiWarps * 32 + 128;  // 384
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+static_assert(kProducerRegs * 128 + kConsumerRegs * kNumEpiWarps * 32 <= 65536, "register split exceeds the SM's file");
 constexpr int kMaxAccCols = 128;                  // accumulator columns per tile: 64 fp32 registers per consumer thread
 constexpr int kABytes = 128 * 128;                // 128 pixels x 32 fp32
 constexpr int kMaxStages = 8;
@@ -259,6 +264,70 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
             }
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ kernel variants
+// The tensor-core conv kernels are compiled per (operand format FMT, BN, MERGED, SPEC, CW) so that every wgmma of their
+// mainloops has a compile-time shape and type.  MERGED = merged split precision: A_hi x [W_hi ; W_lo] at N = 2*BN plus
+// A_lo x W_hi at N = BN into a 2*BN-column accumulator.  Only the combinations igemm_launch can select are instantiated:
+//   merged      16-bit operands and 2*BN <= 128
+//   SPEC 1, 2   SPADE epilogue, so BN % 64 == 0
+//   CW 32       needs 32 | the channels a warp owns per tile (BN/2, SPADE BN/4): BN >= 64, SPADE specialisations BN = 128
+template <int FMT, int BN, bool MERGED, int SPEC, int CW>
+constexpr bool conv_variant_exists() {
+    return (!MERGED || (FMT != 0 && 2 * BN <= kMaxAccCols)) && (SPEC == 0 || BN % 64 == 0) &&
+           (CW == 16 || (SPEC == 0 ? BN >= 64 : BN == 128));
+}
+
+// Calls L::run<FMT, BN, MERGED, SPEC, CW>() for run-time values; run() returns an error status for a combination that
+// conv_variant_exists rejects, and so does this function for values outside the template domain.
+template <int FMT, int BN, bool MERGED, int SPEC, class L>
+int dispatch_cw(const L& l, int cw) {
+    if (cw == 16) return l.template run<FMT, BN, MERGED, SPEC, 16>();
+    if (cw == 32) return l.template run<FMT, BN, MERGED, SPEC, 32>();
+    return set_error(-14, "conv kernel: no variant for epilogue chunk width %d", cw);
+}
+template <int FMT, int BN, bool MERGED, class L>
+int dispatch_spec(const L& l, int spec, int cw) {
+    if (spec == 0) return dispatch_cw<FMT, BN, MERGED, 0>(l, cw);
+    if (spec == 1) return dispatch_cw<FMT, BN, MERGED, 1>(l, cw);
+    if (spec == 2) return dispatch_cw<FMT, BN, MERGED, 2>(l, cw);
+    return set_error(-14, "conv kernel: no variant for epilogue specialisation %d", spec);
+}
+template <int FMT, int BN, class L>
+int dispatch_merged(const L& l, bool merged, int spec, int cw) {
+    return merged ? dispatch_spec<FMT, BN, true>(l, spec, cw) : dispatch_spec<FMT, BN, false>(l, spec, cw);
+}
+template <int FMT, class L>
+int dispatch_bn(const L& l, int bn, bool merged, int spec, int cw) {
+    if (bn == 32) return dispatch_merged<FMT, 32>(l, merged, spec, cw);
+    if (bn == 64) return dispatch_merged<FMT, 64>(l, merged, spec, cw);
+    if (bn == 128) return dispatch_merged<FMT, 128>(l, merged, spec, cw);
+    return set_error(-14, "conv kernel: no variant for BN %d", bn);
+}
+template <class L>
+int dispatch_conv_variant(const L& l, int fmt, int bn, bool merged, int spec, int cw) {
+    if (fmt == 0) return dispatch_bn<0>(l, bn, merged, spec, cw);
+    if (fmt == 1) return dispatch_bn<1>(l, bn, merged, spec, cw);
+    if (fmt == 2) return dispatch_bn<2>(l, bn, merged, spec, cw);
+    return set_error(-14, "conv kernel: no variant for operand format %d", fmt);
+}
+
+// Launches `kernel` with the whole opt-in shared memory, setting the attribute once per device and variant.
+template <class K, class... Args>
+int launch_conv_kernel(K* kernel, int& attr_dev, int grid, size_t smem_bytes, cudaStream_t stream, const Args&... args) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (attr_dev != dev) {
+        const cudaError_t e = cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+        attr_dev = dev;
+    }
+    kernel<<<grid, kThreads, smem_bytes, stream>>>(args...);
+    count_launch();
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error((int)e, "conv kernel launch: %s", cudaGetErrorString(e));
+    return 0;
 }
 
 }  // namespace mg

@@ -10,7 +10,10 @@
 //   accumulator lives in the registers of two consumer warpgroups (rows 0-63 / 64-127 of the tile)
 //   and goes through a shared-memory tile to the epilogue those same 8 warps run; the producer
 //   keeps filling the stage ring meanwhile;
-// * warp roles: warps 0..7 = wgmma consumers + epilogue, warp 8 = TMA producer;
+// * warp roles: warps 0..7 = wgmma consumers + epilogue (232 registers each), warps 8..11 = producer
+//   warpgroup (40 registers; one thread issues the TMA loads);
+// * mainloop: compile-time wgmma shape and format, one wgmma group kept in flight (wait_group 1),
+//   a stage released once the wait that retires its MMAs has passed;
 // * persistent CTAs (<= 1 per SM), static round-robin tile schedule with the N-tile index fastest
 //   so CTAs running concurrently share activation tiles through L2.
 //
@@ -21,6 +24,7 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <type_traits>
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
 #include "mg_ptx.cuh"
@@ -61,14 +65,16 @@ __device__ __forceinline__ void store16(const IgemmParams& p, const float (&y)[1
     }
 }
 
+// FMT (operand format), BN and MERGED fix the shape and type of every wgmma (see conv_variant_exists in mg_epilogue.cuh).
 // SPEC selects a compile-time specialisation of the (instruction-bound) epilogue:
 //   0 generic (everything decided at run time)
 //   1 SPADE + LeakyReLU -> bf16 hi/lo operand only      2 SPADE + no activation -> bf16 hi/lo operand only
 // CW: channels per epilogue chunk (16 or 32), compile time so that the per-chunk register arrays are sized exactly.
-template <int SPEC, int CW>
+template <int FMT, int BN, bool MERGED, int SPEC, int CW>
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB, const IgemmParams p) {
+    constexpr int kAcc = MERGED ? 2 * BN : BN;   // accumulator columns
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // 1024-align the operand ring (SWIZZLE_128B atoms are 1024 B).
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -102,11 +108,16 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int ksteps = p.KH * p.KW * p.parts * p.kchunks;
     const int m_tiles_per_img = p.tiles_w * p.tiles_h;
 
+    if (warp >= kNumEpiWarps) {
+        // The producer warpgroup hands its registers to the consumers; one thread of it issues every TMA load.
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp != kNumEpiWarps || lane != 0) return;
+    }
     if (warp == kNumEpiWarps && p.halo) {
         // ===================== TMA producer, halo mode (one thread) =====================
         // Two rings: A = input patches (one per K chunk [x hi/lo part], reused by all 9 taps), B = weights
         // (one slot per tap).  A patches are prefetched up to a_slots-1 items ahead of the weight stream.
-        if (lane == 0) {
+        {
             const int parts2 = p.merged ? 2 : 1;
             const int bparts = p.merged ? 2 : 1;
             uint8_t* a_ring = smem;
@@ -123,7 +134,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         while (tileA < p.num_tiles && a_issued < b_item + p.a_slots) {
                             const bool must = a_issued <= b_item;
                             if (!must && !mbar_test_wait(&aempty_bar[as_], aphs ^ 1)) break;
-                            if (must) mbar_wait(&aempty_bar[as_], aphs ^ 1);
+                            if (must) mbar_wait_report(&aempty_bar[as_], aphs ^ 1);
                             const int mA = tileA / p.n_tiles;
                             const int twA = mA % p.tiles_w, thA = (mA / p.tiles_w) % p.tiles_h, tnA = mA / m_tiles_per_img;
                             const int kcA = itA / parts2, partA = itA - kcA * parts2;
@@ -134,7 +145,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             if (++itA == p.n_items) { itA = 0; tileA += gridDim.x; }
                             ++a_issued;
                         }
-                        mbar_wait(&empty_bar[bs], bph ^ 1);
+                        mbar_wait_report(&empty_bar[bs], bph ^ 1);
                         uint8_t* sb = b_ring + (size_t)bs * p.b_slot_bytes;
                         const int kofs = tap * bparts * p.Cin + kc * p.kelem;
                         if (p.merged && part == 0) {
@@ -153,7 +164,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
     } else if (warp == kNumEpiWarps) {
         // ===================== TMA producer (one thread) =====================
-        if (lane == 0) {
+        {
             int st = 0;
             uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -176,7 +187,7 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const int bsel = part == 2 ? 1 : 0;
                         const bool both = p.merged && part == 0;
                         for (int kc = 0; kc < p.kchunks; ++kc) {
-                            mbar_wait(&empty_bar[st], ph ^ 1);
+                            mbar_wait_report(&empty_bar[st], ph ^ 1);
                             uint8_t* sa = smem + (size_t)st * stage_bytes;
                             const uint32_t txs = (ldA ? kABytes : 0) + (ldB ? p.BN * 128 * (both ? 2 : 1) : 0);
                             if (txs == 0) { mbar_arrive(&full_bar[st]); }
@@ -195,14 +206,27 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
     } else {
         // ===================== consumers: warpgroup wg multiplies rows 64*wg.. of the tile, then all 8 warps run the epilogue
+        setmaxnreg_inc<kConsumerRegs>();
         const int wg = warp >> 2;
         const int quarter = warp & 3;           // rows 32*quarter.. of the accumulator tile in the epilogue
         const int half = warp >> 2;             // column half handled by this warp in the epilogue
         float* scr = reinterpret_cast<float*>(smem + p.epi_off) + warp * (32 * (CW + 4));
-        float acc[64];
+        float acc[kAcc / 2];
         int st = 0, bs = 0, as_ = 0;
         uint32_t ph = 0, bph = 0, aphs = 0;
         const uint32_t ring = smem_u32(smem);
+        // Pipelined mainloop: one wgmma group stays in flight.  After a step commits, wait_group 1 retires the step before
+        // it, and only then is that step's B slot (classic mode: its whole stage) released; an A patch (halo mode) is
+        // released by the wait that retires its last step.  held_*: slots whose release waits for that retirement.
+        int held_b = -1, held_a = -1;
+        auto release_held = [&]() {
+            __syncwarp();
+            if (lane == 0) {   // this warp's reads of the slots are done
+                if (held_b >= 0) mbar_arrive(&empty_bar[held_b]);
+                if (held_a >= 0) mbar_arrive(&aempty_bar[held_a]);
+            }
+            held_b = held_a = -1;
+        };
         for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
             const int nt = tile % p.n_tiles;
             const int m = tile / p.n_tiles;
@@ -210,56 +234,71 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const int th = (m / p.tiles_w) % p.tiles_h;
             const int tn = m / m_tiles_per_img;
             if (p.halo) {
-                const int parts2 = p.merged ? 2 : 1;
+                constexpr int parts2 = MERGED ? 2 : 1;
                 const uint32_t b_ring = ring + (uint32_t)(p.a_slots * p.patch_bytes);
                 for (int it = 0; it < p.n_items; ++it) {
-                    const int part = it % parts2;
-                    const int n = (p.merged && part == 1) ? p.BN : p.acc_cols;
                     mbar_wait(&afull_bar[as_], aphs);
                     // rows 64.. of the tile are its pixel rows 8.., eight patch rows of PW pixels further on
                     const uint32_t a_base = ring + (uint32_t)(as_ * p.patch_bytes) + (uint32_t)(wg * 8 * p.PW * 128);
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const int kh = tap / 3, kw = tap - kh * 3;
-                        mbar_wait(&full_bar[bs], bph);
-                        // tap (kh, kw) = the same patch read from row kh*PW + kw on; 8-pixel row groups are PW rows apart
-                        const uint32_t a_tap = a_base + (uint32_t)((kh * p.PW + kw) * 128);
-                        const uint64_t db = wg_desc_sw128(b_ring + (uint32_t)(bs * p.b_slot_bytes), 1024);
-                        wgmma_fence();
+                    // the nine taps of one item at MMA width N
+                    auto item = [&](auto n_cols) {
+                        constexpr int N = decltype(n_cols)::value;
+                        for (int tap = 0; tap < 9; ++tap) {
+                            const int kh = tap / 3, kw = tap - kh * 3;
+                            mbar_wait(&full_bar[bs], bph);
+                            // tap (kh, kw) = the same patch read from row kh*PW + kw on; 8-pixel row groups are PW rows apart
+                            const uint32_t a_tap = a_base + (uint32_t)((kh * p.PW + kw) * 128);
+                            const uint64_t db = wg_desc_sw128(b_ring + (uint32_t)(bs * p.b_slot_bytes), 1024);
+                            wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t da = wg_desc_sw128(a_tap + (uint32_t)(k * 32), (uint32_t)(p.PW * 128));
-                            wgmma_k32b(acc, n, p.a_fmt, da, db + (uint64_t)(2 * k), (it | tap | k) != 0 ? 1u : 0u);
+                            for (int k = 0; k < 4; ++k) {
+                                const uint64_t da = wg_desc_sw128(a_tap + (uint32_t)(k * 32), (uint32_t)(p.PW * 128));
+                                wgmma_step<FMT, N>(acc, da, db + (uint64_t)(2 * k), (it | tap | k) != 0 ? 1u : 0u);
+                            }
+                            wgmma_commit();
+                            wgmma_wait<1>();
+                            release_held();
+                            held_b = bs;
+                            if (++bs == p.b_slots) { bs = 0; bph ^= 1; }
                         }
-                        wgmma_commit();
-                        wgmma_wait_all();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&empty_bar[bs]);
-                        if (++bs == p.b_slots) { bs = 0; bph ^= 1; }
-                    }
-                    if (lane == 0) mbar_arrive(&aempty_bar[as_]);
+                    };
+                    // merged split precision: items alternate between A_hi x [W_hi ; W_lo] (N = 2*BN) and A_lo x W_hi (N = BN)
+                    if (MERGED && it % parts2 == 1) item(std::integral_constant<int, BN>{});
+                    else item(std::integral_constant<int, kAcc>{});
+                    held_a = as_;
                     if (++as_ == p.a_slots) { as_ = 0; aphs ^= 1; }
                 }
             } else {
-                for (int ks = 0; ks < ksteps; ++ks) {
-                    mbar_wait(&full_bar[st], ph);
-                    const uint32_t sa = ring + (uint32_t)(st * stage_bytes);
-                    const uint64_t da = wg_desc_sw128(sa + (uint32_t)(wg * 64 * 128), 1024);
-                    const uint64_t db = wg_desc_sw128(sa + kABytes, 1024);
-                    // merged split precision: k-steps alternate (per K-chunk run) between N = 2*BN and N = BN
-                    const int n = (p.merged && ((ks / p.kchunks) & 1)) ? p.BN : p.acc_cols;
-                    wgmma_fence();
+                // one run = the K chunks of one (tap, part) at MMA width N
+                auto run = [&](int ks0, auto n_cols) {
+                    constexpr int N = decltype(n_cols)::value;
+                    for (int ks = ks0; ks < ks0 + p.kchunks; ++ks) {
+                        mbar_wait(&full_bar[st], ph);
+                        const uint32_t sa = ring + (uint32_t)(st * stage_bytes);
+                        const uint64_t da = wg_desc_sw128(sa + (uint32_t)(wg * 64 * 128), 1024);
+                        const uint64_t db = wg_desc_sw128(sa + kABytes, 1024);
+                        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)   // advance 32 B inside the 128 B swizzle row: +2 in 16 B units
-                        wgmma_k32b(acc, n, p.a_fmt, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (ks | k) != 0 ? 1u : 0u);
-                    wgmma_commit();
-                    wgmma_wait_all();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_bar[st]);   // this warp's reads of the stage are done
-                    if (++st == p.stages) { st = 0; ph ^= 1; }
+                        for (int k = 0; k < 4; ++k)   // advance 32 B inside the 128 B swizzle row: +2 in 16 B units
+                            wgmma_step<FMT, N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (ks | k) != 0 ? 1u : 0u);
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        release_held();
+                        held_b = st;
+                        if (++st == p.stages) { st = 0; ph ^= 1; }
+                    }
+                };
+                // merged split precision: runs alternate between N = 2*BN and N = BN
+                for (int ks0 = 0; ks0 < ksteps; ks0 += p.kchunks) {
+                    if (MERGED && ((ks0 / p.kchunks) & 1)) run(ks0, std::integral_constant<int, BN>{});
+                    else run(ks0, std::integral_constant<int, kAcc>{});
                 }
             }
+            wgmma_wait<0>();
+            wgmma_fence_operand(acc);
+            release_held();
             bar_sync(1, kNumEpiWarps * 32);     // the previous tile's epilogue is done with the accumulator tile
-            acc_store(acc_tile, p.acc_ld, acc, p.acc_cols, wg * 64);
+            acc_store(acc_tile, p.acc_ld, acc, kAcc, wg * 64);
             bar_sync(1, kNumEpiWarps * 32);
             if (p.epi_impl == 1) {
                 epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, tw, th, tn, quarter, half, lane);
@@ -397,6 +436,25 @@ igemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------------
+struct IgemmLaunch {
+    const CUtensorMap *tmA, *tmA2, *tmB;
+    const IgemmParams* p;
+    int grid;
+    size_t smem_bytes;
+    cudaStream_t stream;
+    template <int FMT, int BN, bool MERGED, int SPEC, int CW>
+    int run() const {
+        if constexpr (conv_variant_exists<FMT, BN, MERGED, SPEC, CW>()) {
+            static thread_local int attr_dev = -1;
+            return launch_conv_kernel(igemm_tf32_kernel<FMT, BN, MERGED, SPEC, CW>, attr_dev, grid, smem_bytes, stream, *tmA, *tmA2,
+                                      *tmB, *p);
+        } else {
+            return set_error(-14, "mg_conv_igemm: no kernel variant for format %d, BN %d, merged %d, SPEC %d, CW %d", FMT, BN,
+                             (int)MERGED, SPEC, CW);
+        }
+    }
+};
+
 static int next_pow2(int v) {
     int r = 1;
     while (r < v) r <<= 1;
@@ -508,14 +566,17 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
             p.b_slots = (smem_avail - p.a_slots * p.patch_bytes) / p.b_slot_bytes;
             if (p.b_slots > kMaxStages) p.b_slots = kMaxStages;
         }
-        if (p.b_slots < 2) return set_error(-13, "mg_conv_igemm: halo rings do not fit shared memory");
+        // the consumers hold two weight slots (the step in flight and the one being issued): a third keeps the producer busy
+        if (p.b_slots < 3) return set_error(-13, "mg_conv_igemm: halo rings do not fit shared memory");
         ring_bytes = (size_t)p.a_slots * p.patch_bytes + (size_t)p.b_slots * p.b_slot_bytes;
         p.stages = p.b_slots;
     } else {
         int stages = smem_avail / stage_bytes;
         if (stages > kMaxStages) stages = kMaxStages;
         const int stages_cap = tune(TK_STAGES);
-        if (stages_cap > 0 && stages > stages_cap) stages = stages_cap;
+        if (stages_cap > 0 && stages > stages_cap) stages = stages_cap > 3 ? stages_cap : 3;
+        // the consumers hold two stages (the step in flight and the one being issued): a third keeps the producer busy
+        if (stages < 3) return set_error(-13, "mg_conv_igemm: stage ring does not fit shared memory");
         p.stages = stages;
         ring_bytes = (size_t)stages * stage_bytes;
     }
@@ -574,30 +635,11 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
         if (rc) return rc;
     }
     const size_t smem_bytes = ring_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + scratch_bytes + acc_bytes;
-    static thread_local int attr_set_dev = -1;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (attr_set_dev != dev) {
-        cudaError_t e = cudaSuccess;
-        const void* kernels[6] = {(const void*)igemm_tf32_kernel<0, 16>, (const void*)igemm_tf32_kernel<0, 32>, (const void*)igemm_tf32_kernel<1, 16>,
-                                  (const void*)igemm_tf32_kernel<1, 32>, (const void*)igemm_tf32_kernel<2, 16>, (const void*)igemm_tf32_kernel<2, 32>};
-        for (int i = 0; i < 6 && e == cudaSuccess; ++i)
-            e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        attr_set_dev = dev;
-    }
     int grid = num_sms();
     if (a->max_ctas > 0 && a->max_ctas < grid) grid = a->max_ctas;
     if (grid > p.num_tiles) grid = p.num_tiles;
-#define MG_LAUNCH(S, C) igemm_tf32_kernel<S, C><<<grid, kThreads, smem_bytes, stream>>>(tmA, tmA2, tmB, p)
-    if (spec == 1) { if (cw == 32) MG_LAUNCH(1, 32); else MG_LAUNCH(1, 16); }
-    else if (spec == 2) { if (cw == 32) MG_LAUNCH(2, 32); else MG_LAUNCH(2, 16); }
-    else { if (cw == 32) MG_LAUNCH(0, 32); else MG_LAUNCH(0, 16); }
-#undef MG_LAUNCH
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error((int)e, "igemm launch: %s", cudaGetErrorString(e));
-    return 0;
+    const IgemmLaunch l{&tmA, &tmA2, &tmB, &p, grid, smem_bytes, stream};
+    return dispatch_conv_variant(l, p.a_fmt, BN, merged, spec, cw);
 }
 
 }  // namespace mg

@@ -62,16 +62,28 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug traps (cudaErrorLaunchFailure) instead of hanging the GPU box.
+// Bounded waits: a protocol bug traps (cudaErrorLaunchFailure) instead of hanging the GPU.
 #ifndef MG_SPIN_LIMIT
 #define MG_SPIN_LIMIT (1u << 26)
 #endif
+// Call-free: safe between a wgmma issue and its wait.  A function call there (printf) makes ptxas serialise every wgmma of
+// the kernel (C7510), so the consumers of the tensor-core kernels only trap.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
+        if (++spins > MG_SPIN_LIMIT) __trap();
+    }
+}
+// The wait of threads that never have a wgmma in flight (TMA producers, operand builders).  Compiled with -DMG_WAIT_PRINTF
+// it names the barrier before the trap.  That is a debugging build only: ptxas serialises every wgmma of a kernel that
+// contains a call anywhere, even on another warp's path.
+__device__ __forceinline__ void mbar_wait_report(uint64_t* bar, uint32_t parity) {
+    uint32_t spins = 0;
+    while (!mbar_try_wait(bar, parity)) {
         if (++spins > MG_SPIN_LIMIT) {
-            printf("mg: mbarrier timeout blk %d thr %d bar %p parity %u\n", blockIdx.x, threadIdx.x,
-                   (void*)bar, parity);
+#ifdef MG_WAIT_PRINTF
+            printf("mg: mbarrier timeout blk %d thr %d bar %p parity %u\n", blockIdx.x, threadIdx.x, (void*)bar, parity);
+#endif
             __trap();
         }
     }
@@ -121,6 +133,20 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const void* tmap, uint64_
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+// Wait until at most N committed wgmma groups of this warpgroup are still in flight.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// Pins the accumulator registers at this point of the program (no read of them may move above a preceding wait).
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operand(float (&acc)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+}
+// Warp-specialised register budgets: the whole warpgroup gives registers back to / takes them from the SM's pool.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(R)); }
 // Named barrier over `count` threads (the consumer warpgroups hand the accumulator tile to the epilogue through smem).
 __device__ __forceinline__ void bar_sync(int id, int count) {
     asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory");
@@ -232,35 +258,38 @@ __device__ __forceinline__ uint64_t wg_desc_mn_sw128(uint32_t smem_addr, uint32_
     return d;
 }
 
-// acc[0, n/2) += A(64 x K) * B(n x K)^T for one K step of 32 bytes (8 tf32 or 16 fp16/bf16); n = 32, 64 or 128 and
-// fmt 0 tf32, 1 fp16, 2 bf16 are uniform across the warpgroup.  The first n columns of an accumulator live in its first
-// n/2 registers, so a narrower MMA may accumulate into the left part of a wider accumulator.
-__device__ __forceinline__ void wgmma_k32b(float (&acc)[64], int n, int fmt, uint64_t da, uint64_t db, uint32_t scale_d) {
-    float (&a32)[32] = *reinterpret_cast<float (*)[32]>(&acc[0]);
-    float (&a16)[16] = *reinterpret_cast<float (*)[16]>(&acc[0]);
-    if (n == 128) {
-        if (fmt == 0) wgmma_tf32_n128(acc, da, db, scale_d);
-        else if (fmt == 1) wgmma_f16_n128(acc, da, db, scale_d);
-        else wgmma_bf16_n128(acc, da, db, scale_d);
-    } else if (n == 64) {
-        if (fmt == 0) wgmma_tf32_n64(a32, da, db, scale_d);
-        else if (fmt == 1) wgmma_f16_n64(a32, da, db, scale_d);
-        else wgmma_bf16_n64(a32, da, db, scale_d);
+// acc[0, N/2) += A(64 x K) * B(N x K)^T for one K step of 32 bytes (8 tf32 or 16 fp16/bf16); FMT 0 tf32, 1 fp16, 2 bf16.
+// Shape and format are compile-time, so a run of these is straight-line code that ptxas can issue back to back.  The first
+// N columns of an accumulator live in its first N/2 registers, so a narrower MMA accumulates into the left part of a wider one.
+template <int FMT, int N, int R>
+__device__ __forceinline__ void wgmma_step(float (&acc)[R], uint64_t da, uint64_t db, uint32_t scale_d) {
+    static_assert(N == 32 || N == 64 || N == 128, "wgmma N");
+    static_assert(N / 2 <= R, "accumulator narrower than the MMA");
+    float (&d)[N / 2] = *reinterpret_cast<float (*)[N / 2]>(&acc[0]);
+    if constexpr (N == 128) {
+        if constexpr (FMT == 0) wgmma_tf32_n128(d, da, db, scale_d);
+        else if constexpr (FMT == 1) wgmma_f16_n128(d, da, db, scale_d);
+        else wgmma_bf16_n128(d, da, db, scale_d);
+    } else if constexpr (N == 64) {
+        if constexpr (FMT == 0) wgmma_tf32_n64(d, da, db, scale_d);
+        else if constexpr (FMT == 1) wgmma_f16_n64(d, da, db, scale_d);
+        else wgmma_bf16_n64(d, da, db, scale_d);
     } else {
-        if (fmt == 0) wgmma_tf32_n32(a16, da, db, scale_d);
-        else if (fmt == 1) wgmma_f16_n32(a16, da, db, scale_d);
-        else wgmma_bf16_n32(a16, da, db, scale_d);
+        if constexpr (FMT == 0) wgmma_tf32_n32(d, da, db, scale_d);
+        else if constexpr (FMT == 1) wgmma_f16_n32(d, da, db, scale_d);
+        else wgmma_bf16_n32(d, da, db, scale_d);
     }
 }
 
 // This thread's part of a finished 64 x n accumulator -> rows [row0, row0 + 64) of an fp32 [rows][ld] smem tile
 // (wgmma layout: warp w of the warpgroup owns rows 16w..16w+15; register 4j+{0,1} = row lane/4, columns 8j + 2(lane%4) + {0,1},
 // register 4j+{2,3} = the same columns 8 rows further down).
-__device__ __forceinline__ void acc_store(float* tile, int ld, const float (&acc)[64], int n, int row0) {
+template <int R>
+__device__ __forceinline__ void acc_store(float* tile, int ld, const float (&acc)[R], int n, int row0) {
     const int lane = threadIdx.x & 31, wr = (threadIdx.x >> 5) & 3;
     const int r = row0 + wr * 16 + (lane >> 2), c = (lane & 3) * 2;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
+    for (int j = 0; j < R / 4; ++j) {
         if (j * 8 < n) {
             *reinterpret_cast<float2*>(tile + (size_t)r * ld + j * 8 + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
             *reinterpret_cast<float2*>(tile + (size_t)(r + 8) * ld + j * 8 + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);

@@ -259,7 +259,7 @@ seg_mlp_tc_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 lo[t] = make_uint2(pack_bf16x2(v.x - f01.x, v.y - f01.y), pack_bf16x2(v.z - f23.x, v.w - f23.y));
             }
             if (prof) { const long long t1 = clock64(); c_gather += t1 - t0; t0 = t1; }
-            mbar_wait(&a_empty[s], ph ^ 1);
+            mbar_wait_report(&a_empty[s], ph ^ 1);
             if (prof) { const long long t1 = clock64(); c_wait += t1 - t0; t0 = t1; }
             uint8_t* base = a_s + (size_t)s * kSegTileBytes + (size_t)r * 128;
             // K order: 8-byte groups g = 0..31: hi taps 0..8 | lo taps 0..8 | hi taps 0..8 | zeros

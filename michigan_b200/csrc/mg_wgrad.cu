@@ -105,7 +105,7 @@ wgrad_tf32_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
             const int tn = t / (p.tiles_w * p.tiles_h);
             const int ow0 = tw * p.TW, oh0 = th * p.TH, n0 = tn * p.TN;
             if (lane == 0) {
-                mbar_wait(&empty_bar[st], ph ^ 1);
+                mbar_wait_report(&empty_bar[st], ph ^ 1);
                 mbar_arrive_expect_tx(&full_bar[st], tx);
             }
             __syncwarp();
