@@ -31,7 +31,7 @@ const char* mg_last_error(void);
 /* number of kernels this library has launched in the calling process (for bench.py's gpu_launches) */
 long long mg_launch_count(void);
 /* Schedule knobs ("MG_DUAL", "MG_MERGE", "MG_HALO", "MG_HALO_PW", "MG_EPI_IMPL", "MG_EPI_IMPL_SPADE", "MG_EPI_CW16",
- * "MG_EPI_CW_SPADE", "MG_STAGES", "MG_WGRAD_DUAL", "MG_THIN_GEMM", "MG_THIN_WGRAD_LEGACY", "MG_GROUP3", "MG_SEG_TMA", "MG_WGRAD_HALO", "MG_EPI_TMA", "MG_BN_FILL", "MG_EPI_EARLY"): initialised once from the
+ * "MG_EPI_CW_SPADE", "MG_STAGES", "MG_WGRAD_DUAL", "MG_THIN_GEMM", "MG_THIN_WGRAD_LEGACY", "MG_GROUP3", "MG_SEG_TMA", "MG_WGRAD_HALO", "MG_EPI_TMA", "MG_BN_FILL", "MG_EPI_EARLY", "MG_EPI_REG"): initialised once from the
  * environment variable of the same name, changed here by tests and A/B tools.  Unknown name: -2 / -1. */
 int mg_set_tuning(const char* name, int value);
 int mg_get_tuning(const char* name);

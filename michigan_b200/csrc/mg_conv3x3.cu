@@ -43,7 +43,8 @@ struct Conv3Params {
 //   merged split   : hi 9 x [W_hi;W_lo] (N = 2BN), lo 9 x W_hi (N = BN)
 //   3-pass split   : hi 18 = tap x {W_hi, W_lo} (N = BN),   lo 9 x W_hi (N = BN)
 // FMT, BN, MERGED: compile-time wgmma shape and type; SPEC, CW: epilogue specialisation (as igemm_tf32_kernel).
-template <int FMT, int BN, bool MERGED, int SPEC, int CW>
+// REG: epilogue_frag straight from the accumulator registers (CW unused) instead of epilogue_tile through shared memory.
+template <int FMT, int BN, bool MERGED, int SPEC, int CW, bool REG>
 __global__ void __launch_bounds__(kThreads, 1)
 conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                      const __grid_constant__ CUtensorMap tmB, const Conv3Params q) {
@@ -135,7 +136,6 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
         const int wg = warp >> 2;
         const int quarter = warp & 3;
         const int half = warp >> 2;
-        float* scr = reinterpret_cast<float*>(smem + p.epi_off) + warp * (32 * (CW + 4));
         const uint32_t a_base0 = smem_u32(a_ring), b_base0 = smem_u32(b_ring);
         float acc0[kAcc / 2], acc1[kAcc / 2];
         int bs = 0, as_ = 0;
@@ -198,17 +198,28 @@ conv3x3_group_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             wgmma_fence_operand(acc0);
             wgmma_fence_operand(acc1);
             release_held();
-            bar_sync(1, kNumEpiWarps * 32);
-            acc_store(acc_tile, p.acc_ld, acc0, kAcc, wg * 64);
-            bar_sync(1, kNumEpiWarps * 32);
-            epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM, th, tn, quarter, half, lane);
-            bar_sync(1, kNumEpiWarps * 32);
-            acc_store(acc_tile, p.acc_ld, acc1, kAcc, wg * 64);
-            bar_sync(1, kNumEpiWarps * 32);
-            epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM + 1, th, tn, quarter, half, lane);
+            if constexpr (REG) {
+                // each warpgroup finishes its own rows: the two are coupled only through the weight and patch slots
+                epilogue_frag<SPEC, BN, MERGED>(p, acc0, acc1, nt, gw * kGM, th, tn, wg, quarter, lane);
+            } else {
+                float* scr = reinterpret_cast<float*>(smem + p.epi_off) + warp * (32 * (CW + 4));
+                bar_sync(1, kNumEpiWarps * 32);
+                acc_store(acc_tile, p.acc_ld, acc0, kAcc, wg * 64);
+                bar_sync(1, kNumEpiWarps * 32);
+                epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM, th, tn, quarter, half, lane);
+                bar_sync(1, kNumEpiWarps * 32);
+                acc_store(acc_tile, p.acc_ld, acc1, kAcc, wg * 64);
+                bar_sync(1, kNumEpiWarps * 32);
+                epilogue_tile<SPEC, CW>(p, scr, acc_tile, nt, gw * kGM + 1, th, tn, quarter, half, lane);
+            }
         }
     }
 }
+
+// Where the register epilogue is used.  Not for the plain (SPEC 0) epilogue at BN = 128 without merged halves: its 16 channel
+// pairs of side inputs per pixel row do not fit next to both tiles' accumulators (392 B of spills), and on an H100 at 400 W
+// the bf16 layers of that shape ran 13-25 % slower than through shared memory.
+constexpr bool conv3_reg_epilogue(int bn, bool merged, int spec) { return !(bn == 128 && !merged && spec == 0); }
 
 struct Conv3Launch {
     const CUtensorMap *tmA, *tmA2, *tmB;
@@ -216,12 +227,20 @@ struct Conv3Launch {
     int grid;
     size_t smem_bytes;
     cudaStream_t stream;
+    bool reg;   // register epilogue (conv3_reg_epilogue): one variant per (FMT, BN, MERGED, SPEC), dispatched as CW = 16
     template <int FMT, int BN, bool MERGED, int SPEC, int CW>
     int run() const {
         if constexpr (conv_variant_exists<FMT, BN, MERGED, SPEC, CW>()) {
+            if constexpr (CW == 16 && conv3_reg_epilogue(BN, MERGED, SPEC)) {
+                if (reg) {
+                    static thread_local int attr_dev_reg = -1;
+                    return launch_conv_kernel(conv3x3_group_kernel<FMT, BN, MERGED, SPEC, CW, true>, attr_dev_reg, grid, smem_bytes,
+                                              stream, *tmA, *tmA2, *tmB, *q);
+                }
+            }
             static thread_local int attr_dev = -1;
-            return launch_conv_kernel(conv3x3_group_kernel<FMT, BN, MERGED, SPEC, CW>, attr_dev, grid, smem_bytes, stream, *tmA, *tmA2,
-                                      *tmB, *q);
+            return launch_conv_kernel(conv3x3_group_kernel<FMT, BN, MERGED, SPEC, CW, false>, attr_dev, grid, smem_bytes, stream, *tmA,
+                                      *tmA2, *tmB, *q);
         } else {
             return set_error(-14, "conv3x3: no kernel variant for format %d, BN %d, merged %d, SPEC %d, CW %d", FMT, BN, (int)MERGED,
                              SPEC, CW);
@@ -237,7 +256,11 @@ int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw,
     if (!(a->KH == 3 && a->KW == 3 && a->stride == 1 && p.pad_h == 1 && p.pad_w == 1 && a->H == a->OH && a->W == a->OW && p.epi_impl == 1 &&
           a->OW >= 16 && a->OW % 16 == 0 && a->OH >= 16 && p.os == 1))
         return 0;
-    const int acc_bytes = 128 * p.acc_ld * 4;
+    // MG_EPI_REG (default 1): the epilogue runs on the accumulator registers and needs neither the shared-memory accumulator
+    // tile nor the transposition scratch, which leaves room for more weight slots.
+    const bool reg = tune(TK_EPI_REG) != 0 && conv3_reg_epilogue(BN, p.merged != 0, spec);
+    if (reg) { scratch_bytes = 0; cw = 16; }
+    const int acc_bytes = reg ? 0 : 128 * p.acc_ld * 4;
     {
         const int avail0 = 227 * 1024 - 1024 - 512 - scratch_bytes - acc_bytes - kASlots * kPatchBytes;
         if (avail0 / (p.acc_cols * 128) < 3) return 0;
@@ -296,7 +319,7 @@ int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw,
     int grid = num_sms();
     if (a->max_ctas > 0 && a->max_ctas < grid) grid = a->max_ctas;
     if (grid > q.num_groups) grid = q.num_groups;
-    const Conv3Launch l{&tmA, &tmA2, &tmB, &q, grid, smem_bytes, stream};
+    const Conv3Launch l{&tmA, &tmA2, &tmB, &q, grid, smem_bytes, stream, reg};
     const int rc = dispatch_conv_variant(l, p.a_fmt, BN, p.merged != 0, spec, cw);
     return rc == 0 ? 1 : rc;
 }

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
+#include <type_traits>
 #include "mg_ptx.cuh"
 #include "mg_internal.h"
 
@@ -66,6 +67,45 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     return v;
 }
 
+// ---------------------------------------------------------------------------------------------- per-element arithmetic
+// epilogue_tile and epilogue_frag hold an element in different threads but must give it the same bits: both call these.
+// Every product that a later add could absorb is rounded explicitly (__fmul_rn, or fmaf where the fusion is wanted):
+// whether the compiler contracts a plain a * b + c depends on the code around it, which differs between the two epilogues.
+// SPADE, first half: gs = 1 + gamma (gbias1 folds the 1 and gamma's bias); returns (x * rstd + shift) * (1 + gamma).
+__device__ __forceinline__ float epi_spade_mod(float x, float sc, float sh, float g1, float gacc, float& gs) {
+    gs = g1 + gacc;
+    return __fmul_rn(fmaf(x, sc, sh), gs);
+}
+// SPADE, second half: + beta (with its bias), activation.
+__device__ __forceinline__ float epi_spade_out(float m, float bb, float bacc, int act) { return apply_act(m + (bb + bacc), act); }
+// Plain conv: per-pixel scale, bias, residual, activation.
+__device__ __forceinline__ float epi_plain(float a, float ps, float bias, bool has_res, float r, int act) {
+    float y = fmaf(a, ps, bias);
+    if (has_res) y += r;
+    return apply_act(y, act);
+}
+// Background blend: bf where the hair / background masks say so.
+__device__ __forceinline__ float epi_blend(float y, float bfv, float om_hair, float om_back) {
+    return fmaf(om_hair, bfv, __fmul_rn(om_back, y));
+}
+// Per-pixel output multiplier (pmul).
+__device__ __forceinline__ float epi_pmul(float y, float pm) { return __fmul_rn(y, pm); }
+// Two consecutive channels -> packed 16-bit hi and lo = cvt(y - float(hi)); fp16 clamps hi to its finite range.
+__device__ __forceinline__ void epi_split16(float a, float b, int fmt16, uint32_t& hi, uint32_t& lo) {
+    if (fmt16 == 1) {
+        const __half2 h2 = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
+        const float2 hf = __half22float2(h2);
+        const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
+        hi = *reinterpret_cast<const uint32_t*>(&h2);
+        lo = *reinterpret_cast<const uint32_t*>(&l2);
+    } else {
+        const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+        const float2 hf = __bfloat1622float2(h2);
+        const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - hf.x, b - hf.y);
+        hi = *reinterpret_cast<const uint32_t*>(&h2);
+        lo = *reinterpret_cast<const uint32_t*>(&l2);
+    }
+}
 
 // One accumulator tile (128 pixels x BN columns, fp32 [128][ld] in shared memory) through the epilogue, executed by the 8
 // consumer warps together (warp -> row quarter `quarter` = warp & 3 and column half `half`).  Each lane reads one
@@ -182,10 +222,13 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
             for (int j = 0; j < passes; ++j) {
                 if (!((vmask >> j) & 1u) || !ch_ok) continue;
                 const float4 xv = (MG_DBGV(p) & (8 | 64)) ? sc4 : pre[j];
-                const float4 gs = make_float4(g14.x + av[j].x, g14.y + av[j].y, g14.z + av[j].z, g14.w + av[j].w);
+                float4 gs, m;
+                m.x = epi_spade_mod(xv.x, sc4.x, sh4.x, g14.x, av[j].x, gs.x);
+                m.y = epi_spade_mod(xv.y, sc4.y, sh4.y, g14.y, av[j].y, gs.y);
+                m.z = epi_spade_mod(xv.z, sc4.z, sh4.z, g14.z, av[j].z, gs.z);
+                m.w = epi_spade_mod(xv.w, sc4.w, sh4.w, g14.w, av[j].w, gs.w);
                 if (has_aux) *reinterpret_cast<float4*>(p.aux + (size_t)pixo[j] * p.Cout + cch) = gs;
-                av[j] = make_float4(fmaf(xv.x, sc4.x, sh4.x) * gs.x, fmaf(xv.y, sc4.y, sh4.y) * gs.y,
-                                    fmaf(xv.z, sc4.z, sh4.z) * gs.z, fmaf(xv.w, sc4.w, sh4.w) * gs.w);
+                av[j] = m;
             }
             if (p.merged) load_chunk(col + ch_tile + p.BN, bv, true);
         }
@@ -196,20 +239,14 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
             const size_t pix = pixo[j];
             float y[4];
             if (spade) {
-                y[0] = av[j].x + (bb4.x + bv[j].x); y[1] = av[j].y + (bb4.y + bv[j].y);
-                y[2] = av[j].z + (bb4.z + bv[j].z); y[3] = av[j].w + (bb4.w + bv[j].w);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) y[i] = apply_act(y[i], act);
+                y[0] = epi_spade_out(av[j].x, bb4.x, bv[j].x, act); y[1] = epi_spade_out(av[j].y, bb4.y, bv[j].y, act);
+                y[2] = epi_spade_out(av[j].z, bb4.z, bv[j].z, act); y[3] = epi_spade_out(av[j].w, bb4.w, bv[j].w, act);
             } else {
                 const float ps = p.pscale ? __ldg(p.pscale + pix) : 1.f;
-                y[0] = fmaf(av[j].x, ps, bias4.x); y[1] = fmaf(av[j].y, ps, bias4.y);
-                y[2] = fmaf(av[j].z, ps, bias4.z); y[3] = fmaf(av[j].w, ps, bias4.w);
-                if (p.res) {
-                    const float4 rv = pre[j];
-                    y[0] += rv.x; y[1] += rv.y; y[2] += rv.z; y[3] += rv.w;
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) y[i] = apply_act(y[i], act);
+                const bool has_res = p.res != nullptr;
+                const float4 rv = has_res ? pre[j] : bias4;
+                y[0] = epi_plain(av[j].x, ps, bias4.x, has_res, rv.x, act); y[1] = epi_plain(av[j].y, ps, bias4.y, has_res, rv.y, act);
+                y[2] = epi_plain(av[j].z, ps, bias4.z, has_res, rv.z, act); y[3] = epi_plain(av[j].w, ps, bias4.w, has_res, rv.w, act);
                 if (p.bf) {
                     // full-resolution mask coordinates of this output pixel (blend epilogue only)
                     const int rr = quarter * 32 + j * ppp + psub;
@@ -218,13 +255,13 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
                                       (size_t)(tw * p.TW + (rr & (p.TW - 1))) * p.mask_stride;
                     const float om_hair = 1.f - __ldg(p.hair + mp), om_back = 1.f - __ldg(p.back + mp);
                     const float4 bfv = __ldg(reinterpret_cast<const float4*>(p.bf + pix * p.Cout + cch));
-                    y[0] = bfv.x * om_hair + y[0] * om_back; y[1] = bfv.y * om_hair + y[1] * om_back;
-                    y[2] = bfv.z * om_hair + y[2] * om_back; y[3] = bfv.w * om_hair + y[3] * om_back;
+                    y[0] = epi_blend(y[0], bfv.x, om_hair, om_back); y[1] = epi_blend(y[1], bfv.y, om_hair, om_back);
+                    y[2] = epi_blend(y[2], bfv.z, om_hair, om_back); y[3] = epi_blend(y[3], bfv.w, om_hair, om_back);
                 }
                 if (p.pmul) {
                     const float pm = __ldg(p.pmul + pix);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) y[i] *= pm;
+                    for (int i = 0; i < 4; ++i) y[i] = epi_pmul(y[i], pm);
                 }
             }
             if (do_round) {
@@ -242,27 +279,181 @@ __device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* scr, 
             if (has_hi && !((MG_DBGV(p) & (8 | 32)) && y[0] != 12345.f)) {
                 uint32_t hi[2], lo[2];
 #pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const float a = y[2 * i], b = y[2 * i + 1];
-                    if (fmt16 == 1) {
-                        const __half2 h2 = __floats2half2_rn(fminf(fmaxf(a, -65504.f), 65504.f), fminf(fmaxf(b, -65504.f), 65504.f));
-                        const float2 hf = __half22float2(h2);
-                        const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
-                        hi[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                        lo[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                    } else {
-                        const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
-                        const float2 hf = __bfloat1622float2(h2);
-                        const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - hf.x, b - hf.y);
-                        hi[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                        lo[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                    }
-                }
+                for (int i = 0; i < 2; ++i) epi_split16(y[2 * i], y[2 * i + 1], fmt16, hi[i], lo[i]);
                 const size_t eo = pix * p.Cout + cch;
                 *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(p.out_hi) + eo) = make_uint2(hi[0], hi[1]);
                 if (has_lo) *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(p.out_lo) + eo) = make_uint2(lo[0], lo[1]);
             }
         }
+    }
+}
+
+// The rest of the epilogue of one output pair (channels ch, ch + 1 of pixel pix): rounding, fp32 store (or accumulation), 16-bit
+// hi/lo copies.
+template <int SPEC>
+__device__ __forceinline__ void epi_store_pair(const IgemmParams& p, size_t pix, int ch, float y0, float y1) {
+    constexpr bool kS = SPEC == 1 || SPEC == 2;
+    if (!kS && p.round_out != 0) { y0 = round_tf32(y0); y1 = round_tf32(y1); }
+    const size_t eo = pix * p.Cout + ch;
+    if (!kS && p.out != nullptr) {
+        float2* op = reinterpret_cast<float2*>(p.out + eo);
+        if (p.accumulate) {
+            const float2 o = *op;
+            y0 += o.x; y1 += o.y;
+        }
+        *op = make_float2(y0, y1);
+    }
+    if ((kS || p.out_hi != nullptr) && !((MG_DBGV(p) & (8 | 32)) && y0 != 12345.f)) {
+        uint32_t hi, lo;
+        epi_split16(y0, y1, kS ? 2 : p.out16_fmt, hi, lo);
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out_hi) + eo) = hi;
+        if (kS || p.out_lo != nullptr) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out_lo) + eo) = lo;
+    }
+}
+
+// The two finished M tiles of a conv3x3_group_kernel group (TW = 8, TH = 16, TN = 1) straight from the wgmma accumulators:
+// no shared-memory tile, no transposition, no barrier.  Thread (warpgroup wg, warp quarter = warp & 3, lane) holds in acc_t
+// rows 64 wg + 16 quarter + lane/4 + 8h (h = 0, 1) of M tile t, i.e. pixel (ow = 8 (tw0 + t) + lane/4, oh = 16 th + 8 wg +
+// 2 quarter + h), and in register 4j + 2h + e the accumulator column 8j + 2 (lane & 3) + e.  So every thread owns 4 pixels and
+// a fixed set of channel pairs, and what the epilogue combines is in the same thread: SPADE's gamma and beta (columns c and
+// c + BN/2) and the two halves of merged split precision (c and c + BN).  The per-pixel side inputs of a tile (SPADE x or the
+// residual, blend maps, pscale / pmul) are loaded before its arithmetic; the per-channel parameters are read through L1.
+// Same arithmetic as epilogue_tile (the epi_* helpers), so every element gets the same bits.
+template <int SPEC, int BN, bool MERGED, int R>
+__device__ __forceinline__ void epilogue_frag(const IgemmParams& p, const float (&acc0)[R], const float (&acc1)[R], int nt, int tw0,
+                                              int th, int tn, int wg, int quarter, int lane) {
+    constexpr bool kS = SPEC == 1 || SPEC == 2;
+    constexpr int kLo = BN / 8;   // register-group offset of accumulator column c + BN (merged split precision)
+    static_assert(R == (MERGED ? BN : BN / 2), "accumulator registers: 64 x N per warpgroup is N / 2 per thread");
+    const int act = SPEC == 1 ? 2 : (SPEC == 2 ? 0 : p.act);
+    if (MG_DBGV(p) & 4) return;
+    const int c0 = 2 * (lane & 3);
+    // the thread's pixels: [tile][h]
+    size_t pix[2][2], src[2][2];
+    bool ok[2][2];
+#pragma unroll
+    for (int t = 0; t < 2; ++t)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int ow = (tw0 + t) * 8 + (lane >> 2), oh = th * 16 + 8 * wg + 2 * quarter + h, n = tn;
+            ok[t][h] = ow < p.OW && oh < p.OH;
+            pix[t][h] = ((size_t)n * p.OHF + (size_t)oh + p.ooh) * p.OWF + (size_t)ow + p.oow;
+            if (kS || p.epi == 1) src[t][h] = ((size_t)n * p.XH + (oh >> p.x_shift)) * p.XW + (ow >> p.x_shift);
+            else src[t][h] = ((size_t)n * p.RH + (oh >> p.res_shift)) * p.RW + (ow >> p.res_shift);
+        }
+    const bool side_ok = !(MG_DBGV(p) & (8 | 64));
+
+    if constexpr (BN % 64 == 0) {
+        if (kS || p.epi == 1) {
+            // ---- SPADE: out = act((x * rstd + shift) * (1 + gamma) + beta), gamma | beta packed [BN/2 | BN/2]
+            constexpr int J = BN / 16, kBeta = BN / 16;
+            const int ch0 = nt * (BN / 2) + c0;   // channel of accumulator column 8j + c0: ch0 + 8j
+            const bool has_aux = !kS && p.aux != nullptr;
+            float2 xv[2][2][J];
+            auto load_x = [&](auto tc) {
+                constexpr int t = decltype(tc)::value;
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int j = 0; j < J; ++j)
+                        xv[t][h][j] = ok[t][h] && side_ok && ch0 + 8 * j < p.Cout
+                                          ? __ldg(reinterpret_cast<const float2*>(p.x + src[t][h] * p.Cout + ch0 + 8 * j))
+                                          : make_float2(0.f, 0.f);
+            };
+            auto tile = [&](const float (&acc)[R], auto tc) {
+                constexpr int t = decltype(tc)::value;
+#pragma unroll
+                for (int j = 0; j < J; ++j) {
+                    const int ch = ch0 + 8 * j;
+                    if (ch >= p.Cout) continue;
+                    const float2 sc = __ldg(reinterpret_cast<const float2*>(p.nscale + ch));
+                    const float2 sh = __ldg(reinterpret_cast<const float2*>(p.nshift + ch));
+                    const float2 g1 = __ldg(reinterpret_cast<const float2*>(p.gbias1 + ch));
+                    const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bbias + ch));
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (!ok[t][h]) continue;
+                        const float2 x = side_ok ? xv[t][h][j] : sc;
+                        float g[2], b[2], gs[2], y[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            g[e] = acc[4 * j + 2 * h + e];
+                            b[e] = acc[4 * (j + kBeta) + 2 * h + e];
+                            if (MERGED) {
+                                g[e] += acc[4 * (j + kLo) + 2 * h + e];
+                                b[e] += acc[4 * (j + kBeta + kLo) + 2 * h + e];
+                            }
+                        }
+                        y[0] = epi_spade_out(epi_spade_mod(x.x, sc.x, sh.x, g1.x, g[0], gs[0]), bb.x, b[0], act);
+                        y[1] = epi_spade_out(epi_spade_mod(x.y, sc.y, sh.y, g1.y, g[1], gs[1]), bb.y, b[1], act);
+                        if (has_aux) *reinterpret_cast<float2*>(p.aux + pix[t][h] * p.Cout + ch) = make_float2(gs[0], gs[1]);
+                        epi_store_pair<SPEC>(p, pix[t][h], ch, y[0], y[1]);
+                    }
+                }
+            };
+            // SPEC 1/2 have the registers to fetch tile 1's x before tile 0's arithmetic; the generic variant fetches it after
+            load_x(std::integral_constant<int, 0>{});
+            if constexpr (kS) load_x(std::integral_constant<int, 1>{});
+            tile(acc0, std::integral_constant<int, 0>{});
+            if constexpr (!kS) load_x(std::integral_constant<int, 1>{});
+            tile(acc1, std::integral_constant<int, 1>{});
+            return;
+        }
+    }
+    if constexpr (!kS) {
+        // ---- plain conv: out = pmul * blend(act(acc * pscale + bias + res))
+        constexpr int J = BN / 8;
+        const int ch0 = nt * BN + c0;
+        const bool has_res = p.res != nullptr, has_bf = p.bf != nullptr;
+        // one pixel row (tile t, row h) at a time: its side loads first, then its arithmetic
+        auto row = [&](const float (&acc)[R], auto tc, auto hc) {
+            constexpr int t = decltype(tc)::value, h = decltype(hc)::value;
+            if (!ok[t][h]) return;
+            float2 rv[J], bfv[J];
+            const float ps = p.pscale ? __ldg(p.pscale + pix[t][h]) : 1.f;
+            const float pm = p.pmul ? __ldg(p.pmul + pix[t][h]) : 1.f;
+            float om_hair = 0.f, om_back = 0.f;
+            if (has_bf) {
+                const int ow = (tw0 + t) * 8 + (lane >> 2), oh = th * 16 + 8 * wg + 2 * quarter + h;
+                const size_t mp = ((size_t)tn * p.MH + (size_t)oh * p.mask_stride) * p.MW + (size_t)ow * p.mask_stride;
+                om_hair = 1.f - __ldg(p.hair + mp);
+                om_back = 1.f - __ldg(p.back + mp);
+            }
+#pragma unroll
+            for (int j = 0; j < J; ++j) {
+                const bool cok = ch0 + 8 * j < p.Cout;
+                rv[j] = cok && has_res && side_ok ? __ldg(reinterpret_cast<const float2*>(p.res + src[t][h] * p.Cout + ch0 + 8 * j))
+                                                  : make_float2(0.f, 0.f);
+                bfv[j] = cok && has_bf ? __ldg(reinterpret_cast<const float2*>(p.bf + pix[t][h] * p.Cout + ch0 + 8 * j))
+                                       : make_float2(0.f, 0.f);
+            }
+#pragma unroll
+            for (int j = 0; j < J; ++j) {
+                const int ch = ch0 + 8 * j;
+                if (ch >= p.Cout) continue;
+                const float2 bias = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + ch)) : make_float2(0.f, 0.f);
+                float a[2], y[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    a[e] = acc[4 * j + 2 * h + e];
+                    if (MERGED) a[e] += acc[4 * (j + kLo) + 2 * h + e];
+                }
+                y[0] = epi_plain(a[0], ps, bias.x, has_res, rv[j].x, act);
+                y[1] = epi_plain(a[1], ps, bias.y, has_res, rv[j].y, act);
+                if (has_bf) {
+                    y[0] = epi_blend(y[0], bfv[j].x, om_hair, om_back);
+                    y[1] = epi_blend(y[1], bfv[j].y, om_hair, om_back);
+                }
+                if (p.pmul) { y[0] = epi_pmul(y[0], pm); y[1] = epi_pmul(y[1], pm); }
+                epi_store_pair<SPEC>(p, pix[t][h], ch, y[0], y[1]);
+            }
+        };
+        using I0 = std::integral_constant<int, 0>;
+        using I1 = std::integral_constant<int, 1>;
+        row(acc0, I0{}, I0{});
+        row(acc0, I0{}, I1{});
+        row(acc1, I1{}, I0{});
+        row(acc1, I1{}, I1{});
     }
 }
 

@@ -35,6 +35,7 @@ enum TuneKnob {
     TK_EPI_TMA,          // MG_EPI_TMA: accepted, no effect on sm_90a
     TK_BN_FILL,          // MG_BN_FILL: generic convs whose tiles do not fill the SMs use a narrower BN (default 1)
     TK_EPI_EARLY,        // MG_EPI_EARLY: accepted, no effect on sm_90a
+    TK_EPI_REG,          // MG_EPI_REG: epilogue of the 3x3 group kernel on the accumulator registers (default 1), 0 through smem
     TK_COUNT
 };
 int tune(int knob);
