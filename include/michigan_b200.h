@@ -356,6 +356,34 @@ int mg_orient_loss_fwd(const float* img_nchw, const float* bank, const float* la
 int mg_orient_loss_bwd(const float* bank, const unsigned char* idx, const float* dmax_l1, const float* dmax_log, const float* weights2,
                        float* dimg_nchw, int N, int H, int W, void* stream);
 
+/* ---- VGG19 perceptual loss (models/networks/loss.py:178-207 VGGLoss, architecture.py:160-190 VGG19) ----------------------
+ * NHWC tensors, C a multiple of 8, every pointer 16-byte aligned.  16-bit formats: 1 = fp16, 2 = bf16.
+ * mg_maxpool2_nhwc: nn.MaxPool2d(2, 2) of VGG19.features[4,9,18,27] (floor mode: out [N,H/2,W/2,C]); reads exactly one of in32 /
+ *   in16 (the producer conv's fp32 or 16-bit output) and writes out32 and/or out16 (the next conv's operand, round to nearest).
+ *   A window's maximum is its first element in row-major order among equals; NaN propagates (torch's rule).
+ * mg_maxpool2_relu_bwd: backward of ReLU -> max-pool (features[3,4], [8,9], [17,18], [26,27]) in gather form:
+ *   dx = [a > 0] * ((a is its window's arg-max ? dpool : 0) + add), with the arg-max recomputed from the same saved pre-pool
+ *   tensor a (a32 or a16) by the forward's rule; add (nullable, may alias dx32) is a gradient already held for a; rows /
+ *   columns of an odd-sized input outside every window get [a > 0] * add.  Writes dx32 and/or dx16 (bf16, conv_dgrad's dy16).
+ * mg_relu_bwd16: ReLU backward of the layers without a pool: dz = [a > 0] * (dy + add) over n elements (n % 8 == 0), add
+ *   nullable and may alias dz32; writes dz32 and/or dz16 (bf16). */
+int mg_maxpool2_nhwc(const float* in32, const void* in16, int in_fmt, float* out32, void* out16, int out_fmt, int N, int H, int W, int C,
+                     void* stream);
+int mg_maxpool2_relu_bwd(const float* dpool, const float* a32, const void* a16, int a_fmt, const float* add, float* dx32, void* dx16,
+                         int N, int H, int W, int C, void* stream);
+int mg_relu_bwd16(const float* dy, const float* add, const float* a32, const void* a16, int a_fmt, float* dz32, void* dz16, long long n,
+                  void* stream);
+
+/* ---- Lab colour loss (models/networks/loss.py:403-531 LabColorLoss, balance_Lab = False) ----------------------------------
+ * fake, real [N,3,H,W] in [-1,1].  Per pixel: rgb = (img+1)/2, xyz = M rgb / rowsum(M) (loss.py:441-460), f(t) = t^(1/3) if
+ * t > 0.008856 else 7.787 t + 0.137931, a = 500 (f(X) - f(Y)), b = 200 (f(Y) - f(Z)) (loss.py:462-485).
+ * fwd: sums[0] += sum |a_fake - a_real| + |b_fake - b_real| (fp64, caller zeroes) => loss = sums[0] / (2*N*H*W) (loss.py:523).
+ * bwd: dfake = gscale[0] * d sums[0] / d fake (gscale: device float = upstream gradient / (2*N*H*W)); f' is taken branch by
+ *      branch (finite at t = 0), sign(0) = 0 as in nn.L1Loss. */
+int mg_lab_loss_fwd(const float* fake_nchw, const float* real_nchw, double* sums, int N, int H, int W, void* stream);
+int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, const float* gscale, float* dfake_nchw, int N, int H, int W,
+                    void* stream);
+
 /* ---- data-parallel exchange over NVLink peer memory --------------------------------------------------------
  * One-shot all-reduce (sum, in place) of a small fp64 vector: replaces the SyncBN master/slave message passing of
  * sync_batchnorm/comm.py:49-133 + batchnorm.py:105-126 (ReduceAddCoalesced / Broadcast of [sum | sum of squares]).

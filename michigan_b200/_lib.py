@@ -122,6 +122,11 @@ SIGNATURES = {
     "mg_loss_reduce": [_p, _i, _p, _p],
     "mg_loss_reduce_bwd": [_p, _i, _p, _p],
     "mg_loss_term_bytes": [],
+    "mg_maxpool2_nhwc": [_p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _p],
+    "mg_maxpool2_relu_bwd": [_p, _p, _p, _i, _p, _p, _p, _i, _i, _i, _i, _p],
+    "mg_relu_bwd16": [_p, _p, _p, _p, _i, _p, _p, _ll, _p],
+    "mg_lab_loss_fwd": [_p, _p, _p, _i, _i, _i, _p],
+    "mg_lab_loss_bwd": [_p, _p, _p, _p, _i, _i, _i, _p],
     "mg_peer_buffer_bytes": [_i],
     "mg_peer_max_elems": [],
     "mg_peer_allreduce_f64": [_p, _i, _p, _i, _i, C.c_ulonglong, _i, _d, _p, _p],

@@ -1,0 +1,320 @@
+// michigan_b200 — VGG19 perceptual loss and Lab colour loss (sm_90a; reference models/networks/loss.py:178-207 VGGLoss,
+// 403-531 LabColorLoss, architecture.py:160-190 VGG19).
+//
+// The VGG19 convolutions run on the existing kernels (conv_thin for conv1_1, the wgmma implicit-GEMM / 3x3 group kernels for
+// the rest, conv_dgrad / thin_dgrad3 backward) and the five L1 terms on mg_loss_reduce.  What the network adds is here:
+//   mg_maxpool2_nhwc      2x2 / stride 2 max-pool (floor mode) of an fp32 or 16-bit NHWC tensor, writing fp32 and/or the 16-bit
+//                         operand of the next conv;
+//   mg_maxpool2_relu_bwd  its gather-form backward fused with the preceding ReLU's: the arg-max is recomputed from the same saved
+//                         tensor the forward pooled, so both agree bit for bit; fp32 and/or bf16 (conv_dgrad's dy16) out;
+//   mg_relu_bwd16         ReLU backward of the layers without a pool, same outputs;
+//   mg_lab_loss_fwd/bwd   the Lab colour L1 loss over fake and real in one pass; d fake written directly (NCHW).
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include "mg_internal.h"
+
+namespace mg {
+
+// ------------------------------------------------------------------------------------------------ 8-channel vectors
+// Every thread of the pooling / ReLU kernels owns 8 consecutive channels: one 16-byte load of a 16-bit tensor, two of fp32.
+__device__ __forceinline__ void load8(const float* a32, const uint16_t* a16, int fmt, size_t off, float v[8]) {
+    if (a32) {
+        const float4 x = __ldg(reinterpret_cast<const float4*>(a32 + off));
+        const float4 y = __ldg(reinterpret_cast<const float4*>(a32 + off + 4));
+        v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w; v[4] = y.x; v[5] = y.y; v[6] = y.z; v[7] = y.w;
+    } else {
+        const uint4 u = __ldg(reinterpret_cast<const uint4*>(a16 + off));
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint16_t lo = (uint16_t)(w[i] & 0xffffu), hi = (uint16_t)(w[i] >> 16);
+            if (fmt == 1) {
+                v[2 * i] = __half2float(__ushort_as_half(lo)); v[2 * i + 1] = __half2float(__ushort_as_half(hi));
+            } else {
+                v[2 * i] = __bfloat162float(__ushort_as_bfloat16(lo)); v[2 * i + 1] = __bfloat162float(__ushort_as_bfloat16(hi));
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void store8_32(float* p, size_t off, const float v[8]) {
+    *reinterpret_cast<float4*>(p + off) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(p + off + 4) = make_float4(v[4], v[5], v[6], v[7]);
+}
+
+// round to nearest; fp16 clamped to its finite range (the out16 convention of the conv epilogues)
+__device__ __forceinline__ uint16_t to16(float v, int fmt) {
+    if (fmt == 1) return __half_as_ushort(__float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f)));
+    return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+}
+
+__device__ __forceinline__ void store8_16(uint16_t* p, size_t off, const float v[8], int fmt) {
+    uint32_t w[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) w[i] = (uint32_t)to16(v[2 * i], fmt) | ((uint32_t)to16(v[2 * i + 1], fmt) << 16);
+    *reinterpret_cast<uint4*>(p + off) = make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// torch's max_pool2d rule: a later element replaces the running maximum if it is larger or NaN, so ties keep the first
+// element in row-major window order
+__device__ __forceinline__ bool pool_takes(float v, float m) { return v > m || isnan(v); }
+
+// ------------------------------------------------------------------------------------------------ max-pool forward
+__global__ void __launch_bounds__(256) maxpool2_kernel(const float* __restrict__ in32, const uint16_t* __restrict__ in16, int in_fmt,
+                                                       float* __restrict__ out32, uint16_t* __restrict__ out16, int out_fmt, int N,
+                                                       int H, int W, int C, int OH, int OW) {
+    const int cg = C / 8;
+    const long long total = (long long)N * OH * OW * cg;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % cg) * 8;
+        long long r = idx / cg;
+        const int ow = (int)(r % OW); r /= OW;
+        const int oh = (int)(r % OH);
+        const int n = (int)(r / OH);
+        const size_t p00 = (((size_t)n * H + 2 * oh) * W + 2 * ow) * C + c;
+        const size_t offs[4] = {p00, p00 + C, p00 + (size_t)W * C, p00 + (size_t)W * C + C};
+        float m[8], v[8];
+        load8(in32, in16, in_fmt, offs[0], m);
+#pragma unroll
+        for (int k = 1; k < 4; ++k) {
+            load8(in32, in16, in_fmt, offs[k], v);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) m[i] = pool_takes(v[i], m[i]) ? v[i] : m[i];
+        }
+        const size_t o = (size_t)idx * 8;
+        if (out32) store8_32(out32, o, m);
+        if (out16) store8_16(out16, o, m, out_fmt);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ max-pool + ReLU backward
+// One thread per (2x2 window, 8 channels), windows covering the whole input (ceil): the last row / column of an odd-sized
+// input belongs to no pooled window and receives only `add`.  g = (window arg-max ? dpool : 0) + add;  dx = [a > 0] * g.
+__global__ void __launch_bounds__(256) maxpool2_relu_bwd_kernel(const float* __restrict__ dpool, const float* __restrict__ a32,
+                                                                const uint16_t* __restrict__ a16, int a_fmt, const float* add,
+                                                                float* dx32, __nv_bfloat16* __restrict__ dx16, int N, int H, int W,
+                                                                int C) {
+    const int OH = H / 2, OW = W / 2, WH = (H + 1) / 2, WW = (W + 1) / 2;
+    const int cg = C / 8;
+    const long long total = (long long)N * WH * WW * cg;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx % cg) * 8;
+        long long r = idx / cg;
+        const int ww = (int)(r % WW); r /= WW;
+        const int wh = (int)(r % WH);
+        const int n = (int)(r / WH);
+        const bool pooled = wh < OH && ww < OW;
+        float a[4][8];
+        bool have[4];
+        size_t offs[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int y = 2 * wh + (k >> 1), x = 2 * ww + (k & 1);
+            have[k] = y < H && x < W;
+            offs[k] = (((size_t)n * H + y) * W + x) * C + c;
+            if (have[k]) load8(a32, a16, a_fmt, offs[k], a[k]);
+        }
+        float dp[8];
+        int arg[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { dp[i] = 0.f; arg[i] = -1; }
+        if (pooled) {
+            load8(dpool, nullptr, 0, (((size_t)n * OH + wh) * OW + ww) * C + c, dp);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                float m = a[0][i];
+                int best = 0;
+#pragma unroll
+                for (int k = 1; k < 4; ++k)
+                    if (pool_takes(a[k][i], m)) { m = a[k][i]; best = k; }
+                arg[i] = best;
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if (!have[k]) continue;
+            float g[8], ad[8];
+            if (add) load8(add, nullptr, 0, offs[k], ad);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                float t = arg[i] == k ? dp[i] : 0.f;
+                if (add) t += ad[i];
+                g[i] = a[k][i] > 0.f ? t : 0.f;
+            }
+            if (dx32) store8_32(dx32, offs[k], g);
+            if (dx16) store8_16(reinterpret_cast<uint16_t*>(dx16), offs[k], g, 2);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ ReLU backward
+// dz = [a > 0] * (dy + add), over n elements (n % 8 == 0).
+__global__ void __launch_bounds__(256) relu_bwd16_kernel(const float* dy, const float* add, const float* __restrict__ a32,
+                                                         const uint16_t* __restrict__ a16, int a_fmt, float* dz32,
+                                                         __nv_bfloat16* __restrict__ dz16, long long n8) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+        const size_t off = (size_t)i * 8;
+        float a[8], d[8], ad[8], g[8];
+        load8(a32, a16, a_fmt, off, a);
+        load8(dy, nullptr, 0, off, d);
+        if (add) load8(add, nullptr, 0, off, ad);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float t = add ? d[k] + ad[k] : d[k];
+            g[k] = a[k] > 0.f ? t : 0.f;
+        }
+        if (dz32) store8_32(dz32, off, g);
+        if (dz16) store8_16(reinterpret_cast<uint16_t*>(dz16), off, g, 2);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ Lab colour loss
+// loss.py:403-531 (balance_Lab = False): rgb = (img + 1) / 2; xyz = M rgb / rowsum(M); f(t) = t^(1/3) if t > 0.008856 else
+// 7.787 t + 0.137931; a = 500 (f(X) - f(Y)), b = 200 (f(Y) - f(Z)).  L (channel 0) never enters the loss.
+__constant__ float kLabM[3][3] = {{0.412453f, 0.357580f, 0.180423f}, {0.212671f, 0.715160f, 0.072169f}, {0.019334f, 0.119193f, 0.950227f}};
+constexpr float kLabT = 0.008856f;
+
+__device__ __forceinline__ void lab_xyz(const float* img, size_t plane, size_t off, float t[3]) {
+    float rgb[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) rgb[c] = (img[c * plane + off] + 1.f) / 2.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        // the reference divides by the fp32 row sums of M (rgb2xyz: M_tmp.sum(dim=2))
+        const float s = (kLabM[k][0] + kLabM[k][1]) + kLabM[k][2];
+        t[k] = (kLabM[k][0] * rgb[0] + kLabM[k][1] * rgb[1] + kLabM[k][2] * rgb[2]) / s;
+    }
+}
+
+__device__ __forceinline__ float lab_f(float t) { return t > kLabT ? powf(t, 1.f / 3.f) : 7.787f * t + 0.137931f; }
+// f'(t), branch by branch: the cube-root branch is never evaluated at or below the threshold (t = 0 for a saturated pixel)
+__device__ __forceinline__ float lab_df(float t, float ft) { return t > kLabT ? ft / (3.f * t) : 7.787f; }
+__device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
+
+// sums[0] += sum over pixels of |a_fake - a_real| + |b_fake - b_real|  (fp64, caller zeroes)
+__global__ void __launch_bounds__(256) lab_loss_fwd_kernel(const float* __restrict__ fake, const float* __restrict__ real,
+                                                           double* __restrict__ sums, int N, long long HW) {
+    double s = 0.0;
+    const long long total = (long long)N * HW;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const long long n = idx / HW, p = idx - n * HW;
+        float tf[3], tr[3], ff[3], fr[3];
+        lab_xyz(fake + (size_t)n * 3 * HW, (size_t)HW, (size_t)p, tf);
+        lab_xyz(real + (size_t)n * 3 * HW, (size_t)HW, (size_t)p, tr);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { ff[k] = lab_f(tf[k]); fr[k] = lab_f(tr[k]); }
+        const float da = 500.f * (ff[0] - ff[1]) - 500.f * (fr[0] - fr[1]);
+        const float db = 200.f * (ff[1] - ff[2]) - 200.f * (fr[1] - fr[2]);
+        s += (double)fabsf(da) + (double)fabsf(db);
+    }
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    __shared__ double part[8];
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int i = 0; i < 8; ++i) t += part[i];
+        atomicAdd(sums, t);
+    }
+}
+
+// dfake = gscale[0] * d(sum |da| + |db|) / d fake
+__global__ void __launch_bounds__(256) lab_loss_bwd_kernel(const float* __restrict__ fake, const float* __restrict__ real,
+                                                           const float* __restrict__ gscale, float* __restrict__ dfake, int N,
+                                                           long long HW) {
+    const float g = __ldg(gscale);
+    const long long total = (long long)N * HW;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const long long n = idx / HW, p = idx - n * HW;
+        float tf[3], tr[3], ff[3], fr[3];
+        lab_xyz(fake + (size_t)n * 3 * HW, (size_t)HW, (size_t)p, tf);
+        lab_xyz(real + (size_t)n * 3 * HW, (size_t)HW, (size_t)p, tr);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { ff[k] = lab_f(tf[k]); fr[k] = lab_f(tr[k]); }
+        const float sa = sgn(500.f * (ff[0] - ff[1]) - 500.f * (fr[0] - fr[1]));
+        const float sb = sgn(200.f * (ff[1] - ff[2]) - 200.f * (fr[1] - fr[2]));
+        // d/d f(X), f(Y), f(Z), then through f' and the row-normalised M; d rgb / d img = 1/2
+        const float dfk[3] = {500.f * sa, -500.f * sa + 200.f * sb, -200.f * sb};
+        float dt[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) dt[k] = dfk[k] * lab_df(tf[k], ff[k]) / ((kLabM[k][0] + kLabM[k][1]) + kLabM[k][2]);
+        float* o = dfake + (size_t)n * 3 * HW + p;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) o[c * HW] = g * 0.5f * (dt[0] * kLabM[0][c] + dt[1] * kLabM[1][c] + dt[2] * kLabM[2][c]);
+    }
+}
+
+static int grid_for(long long work) {
+    long long g = (work + 255) / 256;
+    const long long cap = (long long)num_sms() * 16;
+    if (g > cap) g = cap;
+    return (int)(g < 1 ? 1 : g);
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+}  // namespace mg
+
+using namespace mg;
+#define ST(s) reinterpret_cast<cudaStream_t>(s)
+
+extern "C" int mg_maxpool2_nhwc(const float* in32, const void* in16, int in_fmt, float* out32, void* out16, int out_fmt, int N, int H,
+                                int W, int C, void* stream) {
+    if ((!in32) == (!in16)) return set_error(-1, "mg_maxpool2_nhwc: exactly one of in32 / in16 must be given");
+    if (!out32 && !out16) return set_error(-1, "mg_maxpool2_nhwc: null output");
+    if ((in16 && (in_fmt < 1 || in_fmt > 2)) || (out16 && (out_fmt < 1 || out_fmt > 2)))
+        return set_error(-3, "mg_maxpool2_nhwc: 16-bit formats are 1 (fp16) or 2 (bf16)");
+    if (N < 1 || H < 2 || W < 2 || C < 8 || C % 8 != 0) return set_error(-2, "mg_maxpool2_nhwc: bad size (C must be a multiple of 8)");
+    if (!aligned16(in32 ? (const void*)in32 : in16) || (out32 && !aligned16(out32)) || (out16 && !aligned16(out16)))
+        return set_error(-4, "mg_maxpool2_nhwc: tensors must be 16-byte aligned");
+    const int OH = H / 2, OW = W / 2;
+    maxpool2_kernel<<<grid_for((long long)N * OH * OW * (C / 8)), 256, 0, ST(stream)>>>(
+        in32, static_cast<const uint16_t*>(in16), in_fmt, out32, static_cast<uint16_t*>(out16), out_fmt, N, H, W, C, OH, OW);
+    return check_launch("mg_maxpool2_nhwc");
+}
+
+extern "C" int mg_maxpool2_relu_bwd(const float* dpool, const float* a32, const void* a16, int a_fmt, const float* add, float* dx32,
+                                    void* dx16, int N, int H, int W, int C, void* stream) {
+    if (!dpool || (!a32) == (!a16)) return set_error(-1, "mg_maxpool2_relu_bwd: need dpool and exactly one of a32 / a16");
+    if (!dx32 && !dx16) return set_error(-1, "mg_maxpool2_relu_bwd: null output");
+    if (a16 && (a_fmt < 1 || a_fmt > 2)) return set_error(-3, "mg_maxpool2_relu_bwd: 16-bit formats are 1 (fp16) or 2 (bf16)");
+    if (N < 1 || H < 2 || W < 2 || C < 8 || C % 8 != 0) return set_error(-2, "mg_maxpool2_relu_bwd: bad size (C must be a multiple of 8)");
+    if (!aligned16(dpool) || !aligned16(a32 ? (const void*)a32 : a16) || (add && !aligned16(add)) || (dx32 && !aligned16(dx32)) ||
+        (dx16 && !aligned16(dx16)))
+        return set_error(-4, "mg_maxpool2_relu_bwd: tensors must be 16-byte aligned");
+    maxpool2_relu_bwd_kernel<<<grid_for((long long)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8)), 256, 0, ST(stream)>>>(
+        dpool, a32, static_cast<const uint16_t*>(a16), a_fmt, add, dx32, static_cast<__nv_bfloat16*>(dx16), N, H, W, C);
+    return check_launch("mg_maxpool2_relu_bwd");
+}
+
+extern "C" int mg_relu_bwd16(const float* dy, const float* add, const float* a32, const void* a16, int a_fmt, float* dz32, void* dz16,
+                             long long n, void* stream) {
+    if (!dy || (!a32) == (!a16)) return set_error(-1, "mg_relu_bwd16: need dy and exactly one of a32 / a16");
+    if (!dz32 && !dz16) return set_error(-1, "mg_relu_bwd16: null output");
+    if (a16 && (a_fmt < 1 || a_fmt > 2)) return set_error(-3, "mg_relu_bwd16: 16-bit formats are 1 (fp16) or 2 (bf16)");
+    if (n < 8 || n % 8 != 0) return set_error(-2, "mg_relu_bwd16: element count must be a positive multiple of 8");
+    if (!aligned16(dy) || !aligned16(a32 ? (const void*)a32 : a16) || (add && !aligned16(add)) || (dz32 && !aligned16(dz32)) ||
+        (dz16 && !aligned16(dz16)))
+        return set_error(-4, "mg_relu_bwd16: tensors must be 16-byte aligned");
+    relu_bwd16_kernel<<<grid_for(n / 8), 256, 0, ST(stream)>>>(dy, add, a32, static_cast<const uint16_t*>(a16), a_fmt, dz32,
+                                                              static_cast<__nv_bfloat16*>(dz16), n / 8);
+    return check_launch("mg_relu_bwd16");
+}
+
+extern "C" int mg_lab_loss_fwd(const float* fake_nchw, const float* real_nchw, double* sums, int N, int H, int W, void* stream) {
+    if (!fake_nchw || !real_nchw || !sums) return set_error(-1, "mg_lab_loss_fwd: null pointer");
+    if (N < 1 || H < 1 || W < 1) return set_error(-2, "mg_lab_loss_fwd: bad size");
+    lab_loss_fwd_kernel<<<grid_for((long long)N * H * W), 256, 0, ST(stream)>>>(fake_nchw, real_nchw, sums, N, (long long)H * W);
+    return check_launch("mg_lab_loss_fwd");
+}
+
+extern "C" int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, const float* gscale, float* dfake_nchw, int N, int H, int W,
+                               void* stream) {
+    if (!fake_nchw || !real_nchw || !gscale || !dfake_nchw) return set_error(-1, "mg_lab_loss_bwd: null pointer");
+    if (N < 1 || H < 1 || W < 1) return set_error(-2, "mg_lab_loss_bwd: bad size");
+    lab_loss_bwd_kernel<<<grid_for((long long)N * H * W), 256, 0, ST(stream)>>>(fake_nchw, real_nchw, gscale, dfake_nchw, N,
+                                                                               (long long)H * W);
+    return check_launch("mg_lab_loss_bwd");
+}

@@ -218,6 +218,96 @@ class _OrientLossFn(torch.autograd.Function):
         return dimg, None, None, None
 
 
+class _VGGLossFn(torch.autograd.Function):
+    """fake || real through VGG19 as one 2N batch; sum_i w_i * mean |x_i - y_i| in one mg_loss_reduce launch; backward: one
+    mg_loss_reduce_bwd launch for the five tap gradients, then the hand-written VGG19 backward down to d fake."""
+
+    @staticmethod
+    def forward(ctx, vgg, weights, fake, real):
+        n = fake.shape[0]
+        x8 = ops.nchw_to_nhwc(torch.cat([fake.detach(), real.detach()], 0).contiguous(), 4)
+        taps, S = vgg.run(x8, n_save=n if ctx.needs_input_grad[2] else 0)
+        del x8
+        pairs = [(t[:n], t[n:]) for t in taps]
+        terms = [_Term(a.data_ptr(), b.data_ptr(), None, a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
+                 for (a, b), w in zip(pairs, weights)]
+        slots = torch.zeros(1, device=fake.device, dtype=torch.float64)
+        _lib.check(_lib.load().mg_loss_reduce(_device_table(terms, fake.device).data_ptr(), len(terms), slots.data_ptr(), ops._stream()),
+                   "mg_loss_reduce")
+        ctx.vgg, ctx.weights, ctx.pairs, ctx.S, ctx.hw = vgg, weights, pairs, S, tuple(fake.shape[2:])
+        return slots.float().reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        pairs = ctx.pairs
+        dev = pairs[0][0].device
+        grads = [torch.empty_like(a) for a, _ in pairs]
+        terms = [_Term(a.data_ptr(), b.data_ptr(), ga.data_ptr(), a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
+                 for (a, b), ga, w in zip(pairs, grads, ctx.weights)]
+        gs = g.reshape(1).contiguous().float()
+        _lib.check(_lib.load().mg_loss_reduce_bwd(_device_table(terms, dev).data_ptr(), len(terms), gs.data_ptr(), ops._stream()),
+                   "mg_loss_reduce_bwd")
+        ctx.pairs = None
+        dimg = ctx.vgg.backward(ctx.S, grads, ctx.hw)
+        ctx.S = None
+        return None, None, dimg, None
+
+
+class VGGLoss(nn.Module):
+    """loss.py:178-207 (remove_background=False): sum_i w_i * L1(vgg(x)_i, vgg(y)_i.detach()), w = 1/32, 1/16, 1/8, 1/4, 1.
+    The image is fed to VGG19 in [-1, 1] without ImageNet normalisation, as the reference does.  The weights are never
+    downloaded (VGG19: `state_dict` or torchvision's cache file)."""
+
+    def __init__(self, opt=None, state_dict=None):
+        super().__init__()
+        if getattr(opt, "remove_background", False):
+            raise NotImplementedError("michigan_b200: --remove_background is not implemented")
+        from .architecture import VGG19
+        self.vgg = VGG19(state_dict=state_dict)
+        self.weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
+        self.opt = opt
+
+    def forward(self, x, y, label=None):
+        dev = x.device
+        if next(self.vgg.parameters()).device != dev:
+            self.vgg.to(dev)
+        if x.shape != y.shape:
+            raise ValueError("VGGLoss: fake %s and real %s differ in shape" % (tuple(x.shape), tuple(y.shape)))
+        return _VGGLossFn.apply(self.vgg, self.weights, x, y.float())
+
+
+class _LabLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, fake, real):
+        f, r = fake.detach().contiguous(), real.detach().contiguous()
+        sums = ops.lab_loss_fwd(f, r)
+        ctx.save_for_backward(f, r)
+        ctx.count = 2 * f.shape[0] * f.shape[2] * f.shape[3]
+        return (sums / ctx.count).float().reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        f, r = ctx.saved_tensors
+        gscale = (g.double() / ctx.count).float().reshape(1).contiguous()
+        return ops.lab_loss_bwd(f, r, gscale), None
+
+
+class LabColorLoss(nn.Module):
+    """loss.py:403-531 with balance_Lab=False: L1 between the a, b channels of the Lab images of fake and real.detach()
+    (xyz2lab of rgb2xyz((img + 1) / 2)), one fused kernel each way (csrc/mg_vgg.cu)."""
+
+    def __init__(self, opt):
+        super().__init__()
+        if getattr(opt, "balance_Lab", False):
+            raise NotImplementedError("michigan_b200: --balance_Lab is not implemented (it needs data/ab_count.npy and grid_sample)")
+        self.opt = opt
+
+    def forward(self, fake, real, mask=None):
+        if fake.shape != real.shape or fake.shape[1] != 3:
+            raise ValueError("LabColorLoss: expected two [N,3,H,W] images, got %s and %s" % (tuple(fake.shape), tuple(real.shape)))
+        return _LabLossFn.apply(fake, real.float())
+
+
 class L1OLoss(nn.Module):
     """loss.py:274-385 with orient_filter='gabor': (orient_loss, confidence_loss) = forward(fake_image, orientation_label,
     input_semantics).  orientation_label: the 1-channel angle map (0..255) or, with --use_ig, the 2-channel (sin 2t, cos 2t) map."""

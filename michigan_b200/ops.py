@@ -472,6 +472,39 @@ def avgpool3s2(x):
     return out
 
 
+def _fmt16(t):
+    """16-bit format code of a tensor (F16 / BF16)."""
+    if t.dtype == torch.float16:
+        return F16
+    if t.dtype == torch.bfloat16:
+        return BF16
+    raise TypeError("expected a float16 or bfloat16 tensor, got %s" % t.dtype)
+
+
+def _split32(a):
+    """fp32 tensor -> (a32, None, 0); 16-bit tensor -> (None, a16, fmt)."""
+    if a.dtype == torch.float32:
+        _chk(a, "a")
+        return a, None, 0
+    fmt = _fmt16(a)
+    _chk(a, "a", a.dtype)
+    return None, a, fmt
+
+
+def maxpool2(x, out16=None, want_f32=True):
+    """2x2 / stride 2 max-pool (floor mode) of an NHWC tensor read as fp32 or 16-bit (x's dtype).
+    out16 = fmt: also write the 16-bit operand of the next conv; returns out32, or (out32|None, out16)."""
+    x32, x16, xfmt = _split32(x)
+    N, H, W, Cc = x.shape
+    out = torch.empty((N, H // 2, W // 2, Cc), device=x.device, dtype=torch.float32) if want_f32 else None
+    o16 = torch.empty((N, H // 2, W // 2, Cc), device=x.device, dtype=_T16[out16]) if out16 is not None else None
+    check(_lib.load().mg_maxpool2_nhwc(_p(x32), _p(x16), xfmt, _p(out), _p(o16), out16 or 0, N, H, W, Cc, _stream()),
+          "mg_maxpool2_nhwc")
+    if out16 is not None:
+        return out, o16
+    return out
+
+
 # ------------------------------------------------------------------------------------------ backward
 def conv_wgrad(dy, x, kh, kw, stride=1, pad=0):
     """Packed weight gradient [Cout][kh*kw*Cin] of an implicit-GEMM conv (tensor cores, split-K)."""
@@ -612,6 +645,55 @@ def act_bwd(dy, y, act, pm1=None, pm2=None, round_tf32=False):
     check(_lib.load().mg_act_bwd(_p(dy), _p(y), _p(dz), dy.numel() // Cc, Cc, act, _p(pm1), _p(pm2), int(round_tf32), _stream()),
           "mg_act_bwd")
     return dz
+
+
+def maxpool2_relu_bwd(dpool, a, add=None, want_f32=True, want16=False):
+    """Backward of y = maxpool2(relu output a): dx = [a > 0] * (pooled gradient routed to each window's arg-max + add).
+    a: the saved tensor the forward pooled (fp32 or 16-bit); add: [N,H,W,C] fp32 or None.
+    -> dx32, or (dx32|None, bf16 copy) with want16."""
+    _chk(dpool, "dpool"); _chk(add, "add")
+    a32, a16, afmt = _split32(a)
+    N, H, W, Cc = a.shape
+    assert tuple(dpool.shape) == (N, H // 2, W // 2, Cc), (dpool.shape, a.shape)
+    dx = torch.empty((N, H, W, Cc), device=a.device, dtype=torch.float32) if want_f32 else None
+    d16 = torch.empty((N, H, W, Cc), device=a.device, dtype=torch.bfloat16) if want16 else None
+    check(_lib.load().mg_maxpool2_relu_bwd(_p(dpool), _p(a32), _p(a16), afmt, _p(add), _p(dx), _p(d16), N, H, W, Cc, _stream()),
+          "mg_maxpool2_relu_bwd")
+    if want16:
+        return dx, d16
+    return dx
+
+
+def relu_bwd16(dy, a, add=None, want_f32=True, want16=False):
+    """dz = [a > 0] * (dy + add) of an NHWC tensor (a fp32 or 16-bit).  -> dz32, or (dz32|None, bf16 copy) with want16."""
+    _chk(dy, "dy"); _chk(add, "add")
+    a32, a16, afmt = _split32(a)
+    assert dy.shape == a.shape, (dy.shape, a.shape)
+    dz = torch.empty(dy.shape, device=dy.device, dtype=torch.float32) if want_f32 else None
+    d16 = torch.empty(dy.shape, device=dy.device, dtype=torch.bfloat16) if want16 else None
+    check(_lib.load().mg_relu_bwd16(_p(dy), _p(add), _p(a32), _p(a16), afmt, _p(dz), _p(d16), dy.numel(), _stream()), "mg_relu_bwd16")
+    if want16:
+        return dz, d16
+    return dz
+
+
+def lab_loss_fwd(fake, real):
+    """-> [1] float64 device tensor: sum over pixels of |a_fake - a_real| + |b_fake - b_real| (NCHW images in [-1, 1])."""
+    _chk(fake, "fake"); _chk(real, "real")
+    N, _, H, W = fake.shape
+    assert fake.shape == real.shape and fake.shape[1] == 3, (fake.shape, real.shape)
+    sums = torch.zeros(1, device=fake.device, dtype=torch.float64)
+    check(_lib.load().mg_lab_loss_fwd(_p(fake), _p(real), _p(sums), N, H, W, _stream()), "mg_lab_loss_fwd")
+    return sums
+
+
+def lab_loss_bwd(fake, real, gscale):
+    """d fake [N,3,H,W] of gscale[0] * lab_loss_fwd(fake, real); gscale: [1] fp32 device tensor."""
+    _chk(fake, "fake"); _chk(real, "real"); _chk(gscale, "gscale")
+    N, _, H, W = fake.shape
+    dfake = torch.empty_like(fake)
+    check(_lib.load().mg_lab_loss_bwd(_p(fake), _p(real), _p(gscale), _p(dfake), N, H, W, _stream()), "mg_lab_loss_bwd")
+    return dfake
 
 
 def instance_norm_act_fwd(x, act=ACT_LRELU, eps=1e-5, round_out=False, pmul=None, out16=None):

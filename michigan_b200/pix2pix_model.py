@@ -2,7 +2,7 @@
 models/pix2pix_model.py (forward 62-122, create_optimizers 124-152, preprocess_input 209-254,
 compute_generator_loss 257-365, compute_discriminator_loss 367-398, generate_fake 505-541,
 discriminate 546-594) for the in-scope configuration: netG=spadeb, netD=multiscale, hinge GAN loss +
-GAN feature loss.  With the reference checkout present, `michigan_b200.install()` lets the reference's
+GAN feature loss, optionally the VGG perceptual, Lab colour and Gabor orientation losses of the README's training command.  With the reference checkout present, `michigan_b200.install()` lets the reference's
 own Pix2PixModel/Pix2PixTrainer drive these networks instead (INTEGRATION.md); this class is the
 stand-alone equivalent used by bench.py and the tests on machines without the reference.
 """
@@ -12,7 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from . import networks, ops
-from .networks.loss import GANFeatLoss, GANLoss
+from .networks.loss import GANFeatLoss, GANLoss, LabColorLoss, VGGLoss
 
 
 class Pix2PixModel(torch.nn.Module):
@@ -32,14 +32,16 @@ class Pix2PixModel(torch.nn.Module):
         if opt.isTrain:
             # The reference's generator objective also contains VGG / style / content / background / rgb / lab / orientation
             # terms, all ON by default (pix2pix_model.py:296-345).  This stand-alone model implements the SURVEY §8d loss set
-            # (hinge GAN + GAN feature matching) plus the Gabor orientation / confidence loss (loss.py:274-385, --no_orient_loss to
-            # drop it): anything else must be switched off explicitly rather than silently dropped.
+            # (hinge GAN + GAN feature matching), the VGG perceptual and Lab colour losses of the README's training command
+            # (--no_vgg_loss / --no_lab_loss to drop them) and the Gabor orientation / confidence loss (loss.py:274-385,
+            # --no_orient_loss): anything else must be switched off explicitly rather than silently dropped.
             # (Through michigan_b200.install() the reference's own Pix2PixModel computes whatever losses it is asked for.)
-            missing = [f for f in ("no_vgg_loss", "no_style_loss", "no_content_loss", "no_background_loss", "no_rgb_loss",
-                                   "no_lab_loss") if not getattr(opt, f, False)]
+            missing = [f for f in ("no_style_loss", "no_content_loss", "no_background_loss", "no_rgb_loss")
+                       if not getattr(opt, f, False)]
             if missing:
-                raise NotImplementedError("michigan_b200.Pix2PixModel trains with the hinge GAN + GAN_Feat losses only; pass --%s "
-                                          "(or drive the reference's Pix2PixModel through michigan_b200.install())" % " --".join(missing))
+                raise NotImplementedError("michigan_b200.Pix2PixModel trains with the hinge GAN, GAN_Feat, VGG, Lab and orientation "
+                                          "losses only; pass --%s (or drive the reference's Pix2PixModel through "
+                                          "michigan_b200.install())" % " --".join(missing))
         self.netIG = None
         if getattr(opt, "use_ig", False):
             self.netIG = networks.define_IG(opt)
@@ -49,6 +51,10 @@ class Pix2PixModel(torch.nn.Module):
         if opt.isTrain:
             self.criterionGAN = GANLoss(opt.gan_mode, opt=opt)
             self.criterionGANFeat = GANFeatLoss(opt)
+            if not getattr(opt, "no_vgg_loss", False):
+                self.criterionVGG = VGGLoss(opt)
+            if not getattr(opt, "no_lab_loss", False):
+                self.criterionLabL1 = LabColorLoss(opt)
             if not getattr(opt, "no_orient_loss", False):
                 from .networks.loss import L1OLoss
                 self.criterionOrient = L1OLoss(opt)
@@ -191,6 +197,11 @@ class Pix2PixModel(torch.nn.Module):
         ref_is_tag = bool(torch.sum(input_tag[:, 1] - input_ref[:, 1]) == 0)
         if self.opt.curr_step == 1 and not self.opt.no_ganFeat_loss and ref_is_tag:
             G_losses["GAN_Feat"] = self.criterionGANFeat(pred_fake, pred_real, label_tag)
+        # pix2pix_model.py:300-307 and 335-340: in the reference's key order (GAN, GAN_Feat, VGG, lab, ORIENT, CONFIDENCE)
+        if self.opt.curr_step == 1 and not getattr(self.opt, "no_vgg_loss", False) and ref_is_tag:
+            G_losses["VGG"] = self.criterionVGG(fake_image, image_tag, label_tag) * self.opt.lambda_vgg
+        if self.opt.curr_step == 1 and not getattr(self.opt, "no_lab_loss", False) and ref_is_tag:
+            G_losses["lab"] = self.criterionLabL1(fake_image, image_tag.detach(), label_tag) * self.opt.lambda_lab
         if not getattr(self.opt, "no_orient_loss", False):
             # pix2pix_model.py:340-347
             orient_loss, confidence_loss = self.criterionOrient(fake_image, orient_mask, input_tag)

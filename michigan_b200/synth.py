@@ -65,6 +65,24 @@ def fill_state_dict(sd, seed=0, power_iters=30):
     return sd
 
 
+def vgg19_state_dict(seed=0):
+    """A deterministic stand-in for the ImageNet VGG19 weights in torchvision's layout (`features.N.{weight,bias}`, the 16 convs
+    of vgg19().features; the classifier is not needed): He-normal weights N(0, 2/fan_in), so that ReLU activations stay O(1)
+    through the 13 convs the perceptual loss uses, and biases N(0, 0.01^2)."""
+    sd, cin, i = {}, 3, 0
+    for v in [64, 64, "M", 128, 128, "M", 256, 256, 256, 256, "M", 512, 512, 512, 512, "M", 512, 512, 512, 512, "M"]:
+        if v == "M":
+            i += 1
+            continue
+        key = "features.%d" % i
+        sd[key + ".weight"] = torch.from_numpy((_rs(seed, key + ".weight").standard_normal((v, cin, 3, 3)) *
+                                                np.sqrt(2.0 / (9 * cin))).astype(np.float32))
+        sd[key + ".bias"] = torch.from_numpy((_rs(seed, key + ".bias").standard_normal(v) * 0.01).astype(np.float32))
+        cin = v
+        i += 2
+    return sd
+
+
 def synthetic_batch(n, size=512, seed=1234, use_ig=False, device="cpu"):
     """The data dict of SURVEY.md §8d: hair = axis-aligned box (~23 % of pixels), ref == tag so that the
     GAN-feature loss is active (pix2pix_model.py:286-297)."""

@@ -1,9 +1,10 @@
 """Per-kernel GPU time of one generator-forward step and one train step at the benchmark configuration (batch 8, 512x512,
 synthetic inputs, random-init weights), from torch.profiler CUDA activity.
 
-    python tools/kernel_times.py OUT_DIR [--batch N] [--warmup W]
+    python tools/kernel_times.py OUT_DIR [--batch N] [--warmup W] [--objective readme]
 
-Writes OUT_DIR/kernel_times.md (one table per workload: kernel, launches, total ms, share of the step's kernel time) and
+--objective readme trains with the loss set of the README's training command (hinge GAN, GAN_Feat, VGG, lab, ORIENT; seeded
+stand-in VGG19 weights) and adds a "train step, paper objective" table.  Writes OUT_DIR/kernel_times.md (one table per workload: kernel, launches, total ms, share of the step's kernel time) and
 OUT_DIR/kernel_times.json.  Templated kernels are listed per instantiation, so the variant of each conv kernel is visible.
 Selects the library like everything else (MICHIGAN_B200_LIB), which makes before/after tables of two builds comparable.
 """
@@ -19,15 +20,30 @@ from torch.profiler import ProfilerActivity, profile
 SIZE = 512
 
 
-def build_model(batch):
+README_LOSSES = dict(no_vgg_loss=False, no_lab_loss=False, no_orient_loss=False)
+
+
+def build_model(batch, **losses):
+    """losses: loss switches over make_opt's defaults (the SURVEY §8d set), e.g. README_LOSSES."""
     import random
+    import tempfile
+    from michigan_b200.networks.architecture import VGG19_WEIGHTS_FILE
     from michigan_b200.options import make_opt
     from michigan_b200.pix2pix_model import Pix2PixModel
-    from michigan_b200.synth import fill_state_dict
+    from michigan_b200.synth import fill_state_dict, vgg19_state_dict
     random.seed(0)
     torch.manual_seed(0)
-    opt = make_opt(is_train=True, gpu_ids=[0], batchSize=batch, niter=50, niter_decay=0)
-    model = Pix2PixModel(opt)
+    opt = make_opt(is_train=True, gpu_ids=[0], batchSize=batch, niter=50, niter_decay=0, **losses)
+    old_hub = torch.hub.get_dir()
+    with tempfile.TemporaryDirectory() as hub:
+        # seeded stand-in VGG19 weights where torchvision keeps its cache (nothing is downloaded)
+        os.makedirs(os.path.join(hub, "checkpoints"))
+        torch.save(vgg19_state_dict(0), os.path.join(hub, "checkpoints", VGG19_WEIGHTS_FILE))
+        torch.hub.set_dir(hub)
+        try:
+            model = Pix2PixModel(opt)
+        finally:
+            torch.hub.set_dir(old_hub)
     fill_state_dict(model.netG.state_dict(), 0)
     fill_state_dict(model.netD.state_dict(), 1)
     model.train()
@@ -64,6 +80,7 @@ def main():
     ap.add_argument("out_dir")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--objective", choices=["8d", "readme"], default="8d")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("kernel_times.py needs a CUDA device")
@@ -82,6 +99,12 @@ def main():
     wrap = DataParallelWithCallback(model, device_ids=[0])
     optG, optD = model.create_optimizers(model.opt)
     tables["train step"] = kernel_table(lambda: train_iteration(wrap, optG, optD, dict(dev)), a.warmup)
+    if a.objective == "readme":
+        del wrap, optG, optD, model
+        model = build_model(a.batch, **README_LOSSES)
+        wrap = DataParallelWithCallback(model, device_ids=[0])
+        optG, optD = model.create_optimizers(model.opt)
+        tables["train step, paper objective"] = kernel_table(lambda: train_iteration(wrap, optG, optD, dict(dev)), a.warmup)
 
     os.makedirs(a.out_dir, exist_ok=True)
     gpu = torch.cuda.get_device_name(0)

@@ -1,0 +1,140 @@
+"""Cost of the paper's objective: the train step with the README's loss set (hinge GAN, GAN_Feat, VGG, lab, ORIENT) against the
+SURVEY §8d set (hinge GAN, GAN_Feat), alternated in one process, plus the VGG and Lab loss kernels on their own and, for
+context, the oracle's VGG restatement run eagerly on CUDA (cuDNN) with the same seeded weights.
+
+    python tools/vgg_lab_time.py OUT_DIR [--batch 8] [--steps 5] [--rounds 3]
+
+Batch 8, 512x512, synthetic inputs.  Writes OUT_DIR/vgg_lab_time.json and prints one line per measurement, headed by the GPU's
+name, power limit and maximum SM clock (read-only nvidia-smi query).  Algorithmic rates: VGG = fake forward + real forward +
+data gradient down to the image (3 x the forward's 2*MAC count per image, computed from the layer shapes); Lab = the bytes
+of both images read by the forward and by the backward plus d fake written.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import torch
+
+SIZE = 512
+_VGG_CFG = [64, 64, "M", 128, 128, "M", 256, 256, 256, 256, "M", 512, 512, 512, 512, "M", 512]
+
+
+def vgg_forward_flop(size):
+    """2 * MAC of VGG19 features[0:30] on one size x size image."""
+    flop, cin, s = 0, 3, size
+    for v in _VGG_CFG:
+        if v == "M":
+            s //= 2
+            continue
+        flop += 2 * 9 * cin * v * s * s
+        cin = v
+    return flop
+
+
+def gpu_info():
+    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], stdout=subprocess.PIPE,
+                       stderr=subprocess.STDOUT, text=True)
+    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "nvidia-smi unavailable"
+
+
+def timed(fn, reps, warmup=2):
+    """Median of `reps` CUDA-event timings of fn() in ms."""
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(reps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        b.synchronize()
+        ts.append(a.elapsed_time(b))
+    return sorted(ts)[len(ts) // 2]
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("out_dir")
+    ap.add_argument("--batch", type=int, default=8)
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--rounds", type=int, default=3)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("vgg_lab_time.py needs a CUDA device")
+    import oracle_vgg_lab as ovl
+    from kernel_times import README_LOSSES, build_model
+    from michigan_b200.networks import LabColorLoss, VGGLoss
+    from michigan_b200.networks.sync_batchnorm import DataParallelWithCallback
+    from michigan_b200.options import make_opt
+    from michigan_b200.pix2pix_model import train_iteration
+    from michigan_b200.synth import synthetic_batch, vgg19_state_dict
+
+    info = gpu_info()
+    print("GPU:", info)
+    n = a.batch
+    data = synthetic_batch(n, SIZE, 1234)
+    dev = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in data.items()}
+    legs = {}
+    for name, losses in (("8d", {}), ("readme", README_LOSSES)):
+        model = build_model(n, **losses)
+        wrap = DataParallelWithCallback(model, device_ids=[0])
+        optG, optD = model.create_optimizers(model.opt)
+        legs[name] = (wrap, optG, optD)
+    res = {"gpu": info, "batch": n, "size": SIZE, "images_per_s": {k: [] for k in legs}}
+    for r in range(a.rounds):
+        for name, (wrap, optG, optD) in legs.items():
+            if r == 0:
+                timed(lambda: train_iteration(wrap, optG, optD, dict(dev)), 1, warmup=2)
+            t = timed(lambda: [train_iteration(wrap, optG, optD, dict(dev)) for _ in range(a.steps)], 1, warmup=0)
+            res["images_per_s"][name].append(1e3 * n * a.steps / t)
+            print("round %d  %-7s train step %.1f ms  %.2f images/s" % (r, name, t / a.steps, 1e3 * n * a.steps / t))
+    del legs, wrap, optG, optD, model
+
+    sd = vgg19_state_dict(0)
+    crit = VGGLoss(make_opt(), state_dict=sd)
+    g = torch.Generator().manual_seed(0)
+    fake = (torch.rand(n, 3, SIZE, SIZE, generator=g) * 2 - 1).cuda()
+    real = (torch.rand(n, 3, SIZE, SIZE, generator=g) * 2 - 1).cuda()
+
+    def vgg_step():
+        x = fake.detach().requires_grad_()
+        crit(x, real).backward()
+
+    flop = 3 * vgg_forward_flop(SIZE) * n
+    ms = timed(vgg_step, 10)
+    res["vgg_ms"], res["vgg_tflops"], res["vgg_gflop_per_image"] = ms, flop / ms / 1e9, flop / n / 1e9
+    print("VGG loss fwd+bwd (ours): %.2f ms, %.1f GFLOP/img, %.0f TFLOP/s algorithmic" % (ms, flop / n / 1e9, flop / ms / 1e9))
+    sdc = {k: v.cuda() for k, v in sd.items()}
+
+    def vgg_oracle():
+        x = fake.detach().requires_grad_()
+        ovl.vgg_loss(x, real, sdc).backward()
+
+    ms_o = timed(vgg_oracle, 5)
+    res["vgg_cudnn_ms"] = ms_o
+    print("VGG loss fwd+bwd (oracle, eager cuDNN, torch defaults): %.2f ms, %.0f TFLOP/s algorithmic" % (ms_o, flop / ms_o / 1e9))
+
+    lab = LabColorLoss(make_opt())
+
+    def lab_step():
+        x = fake.detach().requires_grad_()
+        lab(x, real).backward()
+
+    ms_l = timed(lab_step, 20)
+    nbytes = n * SIZE * SIZE * 4 * (6 + 6 + 3)
+    res["lab_ms"], res["lab_gbs"] = ms_l, nbytes / ms_l / 1e6
+    print("Lab loss fwd+bwd: %.3f ms, %.0f GB/s algorithmic" % (ms_l, nbytes / ms_l / 1e6))
+    os.makedirs(a.out_dir, exist_ok=True)
+    with open(os.path.join(a.out_dir, "vgg_lab_time.json"), "w") as f:
+        json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
