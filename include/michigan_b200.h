@@ -288,7 +288,8 @@ int mg_thin_wgrad(const float* x, const float* dz, float* dwt, int N, int H, int
  *  bias_sums != null: [Cout] doubles += per-channel sums of that dz = the conv's bias gradient; both save a full pass over dz.) */
 int mg_thin_dgrad3(const float* dz, const float* wt, float* dimg_nchw, int N, int H, int W, int CinP, int OH, int OW, int Cout,
                    int KH, int KW, int stride, int pad, int c_lo, void* stream);
-/* conv_img backward: dx [N,H,W,Cin], dw [Cout,Cin,3,3] and db [Cout] are ACCUMULATED (zero them first). */
+/* conv_img backward: dx [N,H,W,Cin] is written; dw [Cout,Cin,3,3] and db [Cout] are ACCUMULATED (zero them first).
+ * Cin must divide 256 and be <= 128 (else -2, before any launch); Cout <= 3. */
 int mg_conv_img_bwd(const float* dy_nchw, const float* y_nchw, const float* x, const float* w, float* dz4_ws, float* dx,
                     float* dw, float* db, int N, int H, int W, int Cin, int Cout, int act_in, int act_out, void* stream);
 int mg_conv_to1_bwd(const float* dl, const float* x, const float* w, float* dx, float* dw, float* db, int N, int H, int W,

@@ -1057,14 +1057,18 @@ extern "C" int mg_thin_dgrad3(const float* dz, const float* wt, float* dimg_nchw
 extern "C" int mg_conv_img_bwd(const float* dy_nchw, const float* y_nchw, const float* x, const float* w, float* dz4_ws, float* dx,
                                float* dw, float* db, int N, int H, int W, int Cin, int Cout, int act_in, int act_out, void* stream) {
     if (!dy_nchw || !y_nchw || !x || !w || !dz4_ws || !dx || !dw) return set_error(-1, "mg_conv_img_bwd: null pointer");
-    if (Cin % 4 != 0 || Cout > 3 || 256 % Cin != 0) return set_error(-2, "mg_conv_img_bwd: Cin must divide 256, Cout<=3");
+    // Cin <= 128: conv_img_wgrad_kernel gives each thread kSlots = 5 of the 9 taps (enough while 256 / Cin >= 2), and its
+    // shared-memory tile (340 * (Cin + 1) + 1024 floats) must fit the 200 KB it requests
+    if (Cin % 4 != 0 || Cin > 128 || Cout > 3 || 256 % Cin != 0)
+        return set_error(-2, "mg_conv_img_bwd: Cin must divide 256 and be <= 128, Cout <= 3");
+    cudaError_t e = cudaFuncSetAttribute(conv_img_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_img_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (e != cudaSuccess) return set_error((int)e, "conv_img_bwd attr: %s", cudaGetErrorString(e));
     conv_img_dz_kernel<<<ew_grid_b((long long)N * H * W), 256, 0, ST(stream)>>>(dy_nchw, y_nchw, dz4_ws, N, Cout, (long long)H * W, act_out);
     count_launch();
-    cudaFuncSetAttribute(conv_img_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     conv_img_dgrad_kernel<<<ew_grid_b((long long)N * H * W * (Cin / 4)), 256, (size_t)9 * 4 * Cin * 4, ST(stream)>>>(dz4_ws, x, w, dx, N, H, W,
                                                                                                                    Cin, Cout, act_in);
     count_launch();
-    cudaFuncSetAttribute(conv_img_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     const int tiles_w = cdivb(W, 32), tiles_h = cdivb(H, 8), num_tiles = tiles_w * tiles_h * N;
     int grid = num_sms() * 2;
     if (grid > num_tiles) grid = num_tiles;
