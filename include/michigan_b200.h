@@ -339,6 +339,7 @@ int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, i
  *   op 0: f = min(sign*a - 1, 0) * (b ? b_i : 1)   hinge, discriminator side (b = weight map)     loss.py:104-120
  *   op 1: f = a                                    generator hinge -mean(D(fake))                  loss.py:123-124
  *   op 2: f = |a - b|                              feature matching, b detached                    loss.py:170-172
+ *   op 3: f = (a - b)^2                            content loss (MSE of relu5_1), b detached       loss.py:662-666
  * mg_loss_reduce_bwd writes ga_i = gslots[out_slot] * scale * df/da for every term with ga != null. */
 int mg_loss_reduce(const void* terms_dev, int n_terms, double* slots, void* stream);
 int mg_loss_reduce_bwd(const void* terms_dev, int n_terms, const float* gslots, void* stream);
@@ -384,6 +385,33 @@ int mg_relu_bwd16(const float* dy, const float* add, const float* a32, const voi
 int mg_lab_loss_fwd(const float* fake_nchw, const float* real_nchw, double* sums, int N, int H, int W, void* stream);
 int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, const float* gscale, float* dfake_nchw, int N, int H, int W,
                     void* stream);
+
+/* ---- style and content losses (models/networks/loss.py:624-711 StyleContentLoss with remove_background = False) ----------
+ * Replaces calc_mean_std (loss.py:624-632), calc_style_loss and calc_content_loss (loss.py:662-683) over the five VGG19 taps.
+ * The per-(n, c) statistics are mg_in_stats' fp64 sums ([N][2][C]: sum x, sum x^2) of each fp32 NHWC tap, one call per tap over
+ * the whole fake || target batch; the content loss is op 3 of mg_loss_reduce.
+ * mg_style_loss_fwd: taps_host: HOST array of n_taps (<= 8) records of mg_style_tap_bytes() bytes, layout
+ *   {const double* sums_f; const double* sums_t; float* coef; long long M; int N, C;}  (M = pixels per image, C % 4 == 0).
+ *   mu = S1 / M, sigma = sqrt((S2 - S1 mu) / (M - 1) + 1e-5) (unbiased variance, as torch.var); in fp64:
+ *   loss[0] += sum over taps of (sum_nc (mu_f - mu_t)^2 + (sigma_f - sigma_t)^2) / (N*C)   (caller zeroes; one block, so the
+ *   sum is bit-reproducible); coef [N][3][C] (16-byte aligned) = fp32 mu_f, mu_f - mu_t, (sigma_f - sigma_t) / sigma_f.
+ *   A tap with M < 2 (relu5_1 of a crop below 32) is refused with -2; the reference returns NaN there.
+ * mg_style_tap_grad: gradient w.r.t. one fake tap x [N, HW, C] (fp32 NHWC, C % 4 == 0, 16-byte aligned), g = device [2] floats
+ *   (upstream gradients of the style and content losses):
+ *   out = add + g[0] (2 (mu_f - mu_t) / (N C HW) + 2 (sigma_f - sigma_t) / (N C sigma_f (HW - 1)) (x - mu_f))
+ *             + g[1] 2 (x - t) / (N C HW)
+ *   coef null drops the style part, content_t (the detached target tap) null the content part; add nullable, may alias out.
+ * ---- background and rgb L1 losses (loss.py:388-400 RGBBackgroundL1Loss, pix2pix_model.py:51,328-333 nn.L1Loss) -------------
+ * fake, tag [N,3,H,W] fp32; mask [N,H,W] (input_semantics[:, 0]) broadcast over the channels, null for the rgb loss.
+ * mg_pixel_l1_fwd: sums[0] += sum |m f - m t| (products rounded first; fp64, caller zeroes) => loss = sums[0] / (3*N*H*W).
+ * mg_pixel_l1_bwd: dfake = (gscale[0] sign(m f - m t)) m, sign(0) = 0 (gscale: device float = upstream gradient / (3*N*H*W)). */
+int mg_style_loss_fwd(const void* taps_host, int n_taps, double* loss, void* stream);
+int mg_style_tap_bytes(void);
+int mg_style_tap_grad(const float* x, const float* coef, const float* content_t, const float* add, float* out, const float* g, int N,
+                      long long HW, int C, void* stream);
+int mg_pixel_l1_fwd(const float* fake_nchw, const float* tag_nchw, const float* mask, double* sums, int N, int H, int W, void* stream);
+int mg_pixel_l1_bwd(const float* fake_nchw, const float* tag_nchw, const float* mask, const float* gscale, float* dfake_nchw, int N,
+                    int H, int W, void* stream);
 
 /* ---- data-parallel exchange over NVLink peer memory --------------------------------------------------------
  * One-shot all-reduce (sum, in place) of a small fp64 vector: replaces the SyncBN master/slave message passing of

@@ -127,6 +127,11 @@ SIGNATURES = {
     "mg_relu_bwd16": [_p, _p, _p, _p, _i, _p, _p, _ll, _p],
     "mg_lab_loss_fwd": [_p, _p, _p, _i, _i, _i, _p],
     "mg_lab_loss_bwd": [_p, _p, _p, _p, _i, _i, _i, _p],
+    "mg_style_loss_fwd": [_p, _i, _p, _p],
+    "mg_style_tap_bytes": [],
+    "mg_style_tap_grad": [_p, _p, _p, _p, _p, _p, _i, _ll, _i, _p],
+    "mg_pixel_l1_fwd": [_p, _p, _p, _p, _i, _i, _i, _p],
+    "mg_pixel_l1_bwd": [_p, _p, _p, _p, _p, _i, _i, _i, _p],
     "mg_peer_buffer_bytes": [_i],
     "mg_peer_max_elems": [],
     "mg_peer_allreduce_f64": [_p, _i, _p, _i, _i, C.c_ulonglong, _i, _d, _p, _p],

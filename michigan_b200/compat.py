@@ -5,9 +5,10 @@ touches arithmetic on the hot path:
      (generator.py:9, normalization.py:13, util/html.py:7-8): stubbed only when they are not installed;
   2. `torch.optim.Adam(betas=(0, 0.9))` with the int 0 (pix2pix_model.py:141-145) is rejected by torch >= 2.x:
      betas are coerced to float;
-  3. `networks.StyleContentLoss` is constructed unconditionally (pix2pix_model.py:47) and downloads VGG19
+  3. `networks.StyleContentLoss` is constructed unconditionally (pix2pix_model.py:47) and needs the VGG19 weights
      (loss.py:659, architecture.py:163): when BOTH --no_style_loss and --no_content_loss are given its result is
-     discarded (pix2pix_model.py:310-319), so it is replaced by a zero stub in that case only.
+     discarded (pix2pix_model.py:310-319), so whatever class is bound (install() binds michigan_b200's) is replaced by a
+     zero stub in that case only.
 """
 import importlib
 import sys

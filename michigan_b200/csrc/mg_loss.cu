@@ -52,6 +52,7 @@ __global__ void edge_weight_kernel(const float* __restrict__ label, float* __res
 //   op 0  hinge, discriminator side: f = min(sign*a - 1, 0) * (w ? w_i : 1)     (loss.py:104-120)
 //   op 1  plain sum: f = a                                                    (generator hinge: -mean(D(fake)), loss.py:123-124)
 //   op 2  L1: f = |a - b|                                                     (GANFeatLoss, loss.py:170-172; b is detached)
+//   op 3  squared difference: f = (a - b)^2                                   (content loss, loss.py:662-666; b is detached)
 struct LossTerm {
     const float* a;
     const float* b;      // op 0: weight map (nullable); op 2: the other tensor
@@ -64,6 +65,9 @@ struct LossTerm {
 // grid.x blocks per term: terms range from 9 K (coarse logits) to 34 M elements (finest feature map) - enough blocks to saturate
 // HBM on the large ones; blocks beyond a small term's size exit immediately
 constexpr int kLossBlocksPerTerm = 592;
+
+// (a - b)^2 with the square rounded before it is summed (no fused multiply-add across terms)
+__device__ __forceinline__ float sq_diff(float a, float b) { const float d = a - b; return __fmul_rn(d, d); }
 
 __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __restrict__ terms, double* __restrict__ slots) {
     const LossTerm t = terms[blockIdx.y];
@@ -78,13 +82,15 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
         if (t.b) b = __ldg(reinterpret_cast<const float4*>(t.b) + i);
         if (t.op == 0) accf += fminf(t.sign * a.x - 1.f, 0.f) * b.x + fminf(t.sign * a.y - 1.f, 0.f) * b.y + fminf(t.sign * a.z - 1.f, 0.f) * b.z + fminf(t.sign * a.w - 1.f, 0.f) * b.w;
         else if (t.op == 1) accf += (a.x + a.y) + (a.z + a.w);
-        else accf += fabsf(a.x - b.x) + fabsf(a.y - b.y) + fabsf(a.z - b.z) + fabsf(a.w - b.w);
+        else if (t.op == 2) accf += fabsf(a.x - b.x) + fabsf(a.y - b.y) + fabsf(a.z - b.z) + fabsf(a.w - b.w);
+        else accf += sq_diff(a.x, b.x) + sq_diff(a.y, b.y) + sq_diff(a.z, b.z) + sq_diff(a.w, b.w);
     }
     for (long long i = n4 * 4 + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
         const float a = __ldg(t.a + i);
         if (t.op == 0) accf += fminf(t.sign * a - 1.f, 0.f) * (t.b ? __ldg(t.b + i) : 1.f);
         else if (t.op == 1) accf += a;
-        else accf += fabsf(a - __ldg(t.b + i));
+        else if (t.op == 2) accf += fabsf(a - __ldg(t.b + i));
+        else accf += sq_diff(a, __ldg(t.b + i));
     }
     double acc = (double)accf;
     for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
@@ -98,7 +104,7 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
     }
 }
 
-// ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * [sign*a - 1 < 0];  op 1: 1;  op 2: sgn(a - b)
+// ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * [sign*a - 1 < 0];  op 1: 1;  op 2: sgn(a - b);  op 3: 2 (a - b)
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
     const LossTerm t = terms[blockIdx.y];
     if (!t.ga) return;
@@ -108,7 +114,8 @@ __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __
         float d;
         if (t.op == 0) d = (t.sign * a - 1.f < 0.f) ? t.sign * (t.b ? __ldg(t.b + i) : 1.f) : 0.f;
         else if (t.op == 1) d = 1.f;
-        else { const float df = a - __ldg(t.b + i); d = df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f); }
+        else if (t.op == 2) { const float df = a - __ldg(t.b + i); d = df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f); }
+        else d = 2.f * (a - __ldg(t.b + i));
         t.ga[i] = g * d;
     }
 }

@@ -8,7 +8,10 @@
 //   mg_maxpool2_relu_bwd  its gather-form backward fused with the preceding ReLU's: the arg-max is recomputed from the same saved
 //                         tensor the forward pooled, so both agree bit for bit; fp32 and/or bf16 (conv_dgrad's dy16) out;
 //   mg_relu_bwd16         ReLU backward of the layers without a pool, same outputs;
-//   mg_lab_loss_fwd/bwd   the Lab colour L1 loss over fake and real in one pass; d fake written directly (NCHW).
+//   mg_lab_loss_fwd/bwd   the Lab colour L1 loss over fake and real in one pass; d fake written directly (NCHW);
+//   mg_style_loss_fwd     the style loss of StyleContentLoss (loss.py:624-711) for every tap in one launch, from mg_in_stats' sums;
+//   mg_style_tap_grad     its gradient w.r.t. one fake tap, with the content loss's folded in at relu5_1, added to the VGG L1's;
+//   mg_pixel_l1_fwd/bwd   the background (masked) and rgb L1 losses on the images (loss.py:388-400, pix2pix_model.py:328-333).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -246,6 +249,150 @@ __global__ void __launch_bounds__(256) lab_loss_bwd_kernel(const float* __restri
     }
 }
 
+// ------------------------------------------------------------------------------------------------ style loss
+// calc_mean_std (loss.py:624-632) from the fp64 per-(n, c) sums of mg_in_stats ([N][2][C]: sum x, then sum x^2, over M pixels):
+//   mu = S1 / M,  var = (S2 - S1 mu) / (M - 1) (unbiased; clamped at 0 against cancellation),  sigma = sqrt(var + 1e-5).
+// calc_style_loss (loss.py:668-683, remove_background False) of one tap: MSE(mu_f, mu_t) + MSE(sigma_f, sigma_t) over N x C.
+struct StyleTap {
+    const double* sums_f;   // [N][2][C] of the fake images
+    const double* sums_t;   // [N][2][C] of the style targets
+    float* coef;            // [N][3][C] out: mu_f, mu_f - mu_t, (sigma_f - sigma_t) / sigma_f
+    long long M;
+    int N, C;
+};
+constexpr int kMaxStyleTaps = 8;
+struct StyleTaps {
+    StyleTap t[kMaxStyleTaps];
+    int n;
+};
+constexpr double kStyleEps = 1e-5;
+
+// One block for every tap (N*C is at most a few thousand per tap): the per-tap sums are added in a fixed order, so the loss is
+// bit-reproducible.  loss[0] += sum over taps of (sum (mu_f - mu_t)^2 + (sigma_f - sigma_t)^2) / (N*C).
+__global__ void __launch_bounds__(512) style_loss_fwd_kernel(const StyleTaps taps, double* __restrict__ loss) {
+    __shared__ double part[16];
+    double total = 0.0;
+    for (int k = 0; k < taps.n; ++k) {
+        const StyleTap t = taps.t[k];
+        const int NC = t.N * t.C;
+        const double M = (double)t.M;
+        double s = 0.0;
+        for (int i = threadIdx.x; i < NC; i += blockDim.x) {
+            const int n = i / t.C, c = i - n * t.C;
+            const double* f = t.sums_f + (size_t)n * 2 * t.C;
+            const double* r = t.sums_t + (size_t)n * 2 * t.C;
+            const double mf = f[c] / M, mt = r[c] / M;
+            const double sf = sqrt(fmax((f[t.C + c] - f[c] * mf) / (M - 1.0), 0.0) + kStyleEps);
+            const double st = sqrt(fmax((r[t.C + c] - r[c] * mt) / (M - 1.0), 0.0) + kStyleEps);
+            const double dm = mf - mt, ds = sf - st;
+            s += dm * dm + ds * ds;
+            float* co = t.coef + (size_t)n * 3 * t.C + c;
+            co[0] = (float)mf;
+            co[t.C] = (float)dm;
+            co[2 * t.C] = (float)(ds / sf);
+        }
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double b = 0.0;
+            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) b += part[w];
+            total += b / (double)NC;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) loss[0] += total;
+}
+
+// Gradient w.r.t. one fake tap [N, HW, C] (4 channels per thread, 128-bit loads and stores):
+//   out = add + g_s [ka (mu_f - mu_t) + kb (sigma_f - sigma_t) / sigma_f (x - mu_f)] + g_c kc (x - t)
+// ka = 2 / (N C M), kb = 2 / (N C (M - 1)), kc = 2 / numel; the style part is skipped without coef, the content part without t.
+// add may alias out (each element is read before it is written by the same thread).
+__global__ void __launch_bounds__(256) style_tap_grad_kernel(const float* __restrict__ x, const float* __restrict__ coef,
+                                                             const float* __restrict__ tgt, const float* add, float* out,
+                                                             const float* __restrict__ g, long long HW, int C, float ka, float kb,
+                                                             float kc, long long total4) {
+    const float gs = coef ? __ldg(g) : 0.f, gc = tgt ? __ldg(g + 1) : 0.f;
+    const int c4 = C / 4;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % c4) * 4;
+        const long long n = i / (HW * c4);
+        const float4 xv = __ldg(reinterpret_cast<const float4*>(x) + i);
+        const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+        float r[4] = {0.f, 0.f, 0.f, 0.f};
+        if (add) {
+            const float4 a = reinterpret_cast<const float4*>(add)[i];
+            r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w;
+        }
+        if (coef) {
+            const float* co = coef + (size_t)n * 3 * C + c;
+            const float4 mu = __ldg(reinterpret_cast<const float4*>(co));
+            const float4 dm = __ldg(reinterpret_cast<const float4*>(co + C));
+            const float4 ds = __ldg(reinterpret_cast<const float4*>(co + 2 * C));
+            const float m[4] = {mu.x, mu.y, mu.z, mu.w}, a[4] = {dm.x, dm.y, dm.z, dm.w}, b[4] = {ds.x, ds.y, ds.z, ds.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) r[j] += gs * (ka * a[j] + kb * b[j] * (xs[j] - m[j]));
+        }
+        if (tgt) {
+            const float4 tv = __ldg(reinterpret_cast<const float4*>(tgt) + i);
+            const float ts[4] = {tv.x, tv.y, tv.z, tv.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) r[j] += gc * (kc * (xs[j] - ts[j]));
+        }
+        reinterpret_cast<float4*>(out)[i] = make_float4(r[0], r[1], r[2], r[3]);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ pixel L1 (background / rgb)
+// RGBBackgroundL1Loss (loss.py:388-400): L1(fake * m, tag * m), m = input_semantics[:, 0] broadcast over the 3 channels; the rgb
+// loss (pix2pix_model.py:51, 328-333) is the same without m.  Both products are rounded before the difference, as torch does.
+__device__ __forceinline__ float pixel_diff(float f, float t, const float* m, size_t mi) {
+    if (!m) return f - t;
+    const float mv = __ldg(m + mi);
+    return __fmul_rn(f, mv) - __fmul_rn(t, mv);
+}
+
+__global__ void __launch_bounds__(256) pixel_l1_fwd_kernel(const float* __restrict__ fake, const float* __restrict__ tag,
+                                                           const float* __restrict__ mask, double* __restrict__ sums, int N,
+                                                           long long HW) {
+    double s = 0.0;
+    const long long total = (long long)N * HW;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const long long n = idx / HW, p = idx - n * HW;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const size_t o = ((size_t)n * 3 + c) * HW + p;
+            s += (double)fabsf(pixel_diff(__ldg(fake + o), __ldg(tag + o), mask, (size_t)idx));
+        }
+    }
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    __shared__ double part[8];
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int i = 0; i < 8; ++i) t += part[i];
+        atomicAdd(sums, t);
+    }
+}
+
+// dfake = (gscale[0] * sign(m f - m t)) * m, sign(0) = 0
+__global__ void __launch_bounds__(256) pixel_l1_bwd_kernel(const float* __restrict__ fake, const float* __restrict__ tag,
+                                                           const float* __restrict__ mask, const float* __restrict__ gscale,
+                                                           float* __restrict__ dfake, int N, long long HW) {
+    const float g = __ldg(gscale);
+    const long long total = (long long)N * HW;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        const long long n = idx / HW, p = idx - n * HW;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const size_t o = ((size_t)n * 3 + c) * HW + p;
+            const float d = g * sgn(pixel_diff(__ldg(fake + o), __ldg(tag + o), mask, (size_t)idx));
+            dfake[o] = mask ? d * __ldg(mask + idx) : d;
+        }
+    }
+}
+
 static int grid_for(long long work) {
     long long g = (work + 255) / 256;
     const long long cap = (long long)num_sms() * 16;
@@ -318,3 +465,56 @@ extern "C" int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, c
                                                                                (long long)H * W);
     return check_launch("mg_lab_loss_bwd");
 }
+
+extern "C" int mg_style_loss_fwd(const void* taps_host, int n_taps, double* loss, void* stream) {
+    if (!taps_host || !loss) return set_error(-1, "mg_style_loss_fwd: null pointer");
+    if (n_taps < 1 || n_taps > kMaxStyleTaps) return set_error(-2, "mg_style_loss_fwd: bad tap count %d", n_taps);
+    StyleTaps taps;
+    taps.n = n_taps;
+    for (int k = 0; k < n_taps; ++k) {
+        const StyleTap& t = static_cast<const StyleTap*>(taps_host)[k];
+        if (!t.sums_f || !t.sums_t || !t.coef) return set_error(-1, "mg_style_loss_fwd: null pointer in tap %d", k);
+        if (t.N < 1 || t.C < 4 || t.C % 4 != 0) return set_error(-2, "mg_style_loss_fwd: bad size in tap %d", k);
+        if (t.M < 2)
+            return set_error(-2, "mg_style_loss_fwd: tap %d has %lld pixel(s); the unbiased variance needs at least 2 (crop size >= 32)", k,
+                             t.M);
+        if (!aligned16(t.coef)) return set_error(-4, "mg_style_loss_fwd: coefficient table of tap %d must be 16-byte aligned", k);
+        taps.t[k] = t;
+    }
+    style_loss_fwd_kernel<<<1, 512, 0, ST(stream)>>>(taps, loss);
+    return check_launch("mg_style_loss_fwd");
+}
+
+extern "C" int mg_style_tap_grad(const float* x, const float* coef, const float* content_t, const float* add, float* out, const float* g,
+                                 int N, long long HW, int C, void* stream) {
+    if (!x || !out || !g) return set_error(-1, "mg_style_tap_grad: null pointer");
+    if (!coef && !content_t) return set_error(-1, "mg_style_tap_grad: neither a style nor a content term");
+    if (N < 1 || C < 4 || C % 4 != 0) return set_error(-2, "mg_style_tap_grad: bad size (C must be a multiple of 4)");
+    if (coef && HW < 2) return set_error(-2, "mg_style_tap_grad: the style term needs at least 2 pixels");
+    if (!aligned16(x) || !aligned16(out) || (coef && !aligned16(coef)) || (content_t && !aligned16(content_t)) || (add && !aligned16(add)))
+        return set_error(-4, "mg_style_tap_grad: tensors must be 16-byte aligned");
+    const double nc = (double)N * C;
+    const float ka = (float)(2.0 / (nc * (double)HW)), kb = (float)(2.0 / (nc * (double)(HW - 1)));
+    const long long total4 = (long long)N * HW * (C / 4);
+    style_tap_grad_kernel<<<grid_for(total4), 256, 0, ST(stream)>>>(x, coef, content_t, add, out, g, HW, C, ka, kb, ka, total4);
+    return check_launch("mg_style_tap_grad");
+}
+
+extern "C" int mg_pixel_l1_fwd(const float* fake_nchw, const float* tag_nchw, const float* mask, double* sums, int N, int H, int W,
+                               void* stream) {
+    if (!fake_nchw || !tag_nchw || !sums) return set_error(-1, "mg_pixel_l1_fwd: null pointer");
+    if (N < 1 || H < 1 || W < 1) return set_error(-2, "mg_pixel_l1_fwd: bad size");
+    pixel_l1_fwd_kernel<<<grid_for((long long)N * H * W), 256, 0, ST(stream)>>>(fake_nchw, tag_nchw, mask, sums, N, (long long)H * W);
+    return check_launch("mg_pixel_l1_fwd");
+}
+
+extern "C" int mg_pixel_l1_bwd(const float* fake_nchw, const float* tag_nchw, const float* mask, const float* gscale, float* dfake_nchw,
+                               int N, int H, int W, void* stream) {
+    if (!fake_nchw || !tag_nchw || !gscale || !dfake_nchw) return set_error(-1, "mg_pixel_l1_bwd: null pointer");
+    if (N < 1 || H < 1 || W < 1) return set_error(-2, "mg_pixel_l1_bwd: bad size");
+    pixel_l1_bwd_kernel<<<grid_for((long long)N * H * W), 256, 0, ST(stream)>>>(fake_nchw, tag_nchw, mask, gscale, dfake_nchw, N,
+                                                                               (long long)H * W);
+    return check_launch("mg_pixel_l1_bwd");
+}
+
+extern "C" int mg_style_tap_bytes(void) { return (int)sizeof(mg::StyleTap); }

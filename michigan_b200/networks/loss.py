@@ -5,6 +5,9 @@ remove_background=False), evaluated by the fused reduction kernels of csrc/mg_lo
   * every call = ONE forward launch (all discriminator scales / all eight feature terms through a descriptor table,
     fp64 accumulation) and ONE backward launch, instead of ~10 eager ops per scale and per term;
   * the wide-edge weight map (loss.py:60-78) is one kernel per scale, cached per (label, size) within an iteration.
+
+The rest of the generator objective follows: the Gabor orientation loss, VGGLoss / StyleContentLoss (every VGG19 term from one
+pass, _VGGObjectiveFn), LabColorLoss, RGBBackgroundL1Loss and the rgb L1 (RGBL1Loss).
 """
 import ctypes as C
 
@@ -19,7 +22,7 @@ class _Term(C.Structure):
                 ("sign", C.c_float), ("op", C.c_int32), ("out_slot", C.c_int32)]
 
 
-OP_HINGE_D, OP_SUM, OP_L1 = 0, 1, 2
+OP_HINGE_D, OP_SUM, OP_L1, OP_SQ = 0, 1, 2, 3
 _table_cache = {}
 
 
@@ -218,39 +221,114 @@ class _OrientLossFn(torch.autograd.Function):
         return dimg, None, None, None
 
 
-class _VGGLossFn(torch.autograd.Function):
-    """fake || real through VGG19 as one 2N batch; sum_i w_i * mean |x_i - y_i| in one mg_loss_reduce launch; backward: one
-    mg_loss_reduce_bwd launch for the five tap gradients, then the hand-written VGG19 backward down to d fake."""
+VGG_WEIGHTS = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
+
+
+def style_min_size_error(h, w):
+    """The style loss's unbiased variance needs at least 2 pixels at relu5_1 (h/16 x w/16); the reference returns NaN below."""
+    if (h // 16) * (w // 16) < 2:
+        return NotImplementedError("michigan_b200: the style loss needs at least 2 pixels at relu5_1 (crop_size >= 32), got %dx%d"
+                                   % (h, w))
+    return None
+
+
+class _VGGObjectiveFn(torch.autograd.Function):
+    """Every VGG19 term of the generator objective from ONE VGG19 forward over fake || tag (|| style image) and ONE backward:
+
+      l1       VGGLoss: sum_i w_i * mean |fake_i - tag_i|               mg_loss_reduce op 2, slot 0
+      content  StyleContentLoss's loss_c: mean (fake_5 - tag_5)^2       mg_loss_reduce op 3, slot 1 (same launch)
+      style    StyleContentLoss's loss_s: sum_i MSE(mu_i) + MSE(sigma_i) of fake against the style image, one mg_in_stats per tap
+               over the whole batch, then one mg_style_loss_fwd launch for the five taps
+
+    want = (l1, content, style); a term not asked for returns None.  style_img None: the style targets are the tag half (2N
+    batch).  Backward: mg_loss_reduce_bwd writes the L1 tap gradients, mg_style_tap_grad adds the style gradient (and at relu5_1
+    the content gradient) in place, then the hand-written VGG19 backward takes them down to d fake."""
 
     @staticmethod
-    def forward(ctx, vgg, weights, fake, real):
+    def forward(ctx, vgg, weights, want, fake, tag, style_img):
+        l1, content, style = want
         n = fake.shape[0]
-        x8 = ops.nchw_to_nhwc(torch.cat([fake.detach(), real.detach()], 0).contiguous(), 4)
-        taps, S = vgg.run(x8, n_save=n if ctx.needs_input_grad[2] else 0)
+        parts = [fake.detach(), tag.detach()] + ([style_img.detach()] if style and style_img is not None else [])
+        x8 = ops.nchw_to_nhwc(torch.cat(parts, 0).contiguous(), 4)
+        taps, S = vgg.run(x8, n_save=n if ctx.needs_input_grad[3] else 0)
         del x8
-        pairs = [(t[:n], t[n:]) for t in taps]
-        terms = [_Term(a.data_ptr(), b.data_ptr(), None, a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
-                 for (a, b), w in zip(pairs, weights)]
-        slots = torch.zeros(1, device=fake.device, dtype=torch.float64)
-        _lib.check(_lib.load().mg_loss_reduce(_device_table(terms, fake.device).data_ptr(), len(terms), slots.data_ptr(), ops._stream()),
-                   "mg_loss_reduce")
-        ctx.vgg, ctx.weights, ctx.pairs, ctx.S, ctx.hw = vgg, weights, pairs, S, tuple(fake.shape[2:])
-        return slots.float().reshape(())
+        pairs = [(t[:n], t[n:2 * n]) for t in taps]
+        out_l1 = out_c = out_s = None
+        if l1 or content:
+            terms = [_Term(a.data_ptr(), b.data_ptr(), None, a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
+                     for (a, b), w in zip(pairs, weights)] if l1 else []
+            if content:
+                a, b = pairs[4]
+                terms.append(_Term(a.data_ptr(), b.data_ptr(), None, a.numel(), 1.0 / a.numel(), 1.0, OP_SQ, 1))
+            slots = torch.zeros(2 if content else 1, device=fake.device, dtype=torch.float64)
+            _lib.check(_lib.load().mg_loss_reduce(_device_table(terms, fake.device).data_ptr(), len(terms), slots.data_ptr(),
+                                                  ops._stream()), "mg_loss_reduce")
+            if content:
+                vals = slots.float()
+                out_l1, out_c = (vals[0] if l1 else None), vals[1]
+            else:
+                out_l1 = slots.float().reshape(())
+        coefs = None
+        if style:
+            t0 = n if style_img is None else 2 * n
+            sums = [ops.channel_sums(t) for t in taps]
+            loss, coefs = ops.style_loss_fwd([(s[:n], s[t0:t0 + n], t.shape[1] * t.shape[2]) for s, t in zip(sums, taps)])
+            out_s = loss.float().reshape(())
+        ctx.vgg, ctx.weights, ctx.want, ctx.pairs, ctx.coefs, ctx.S, ctx.hw = vgg, weights, want, pairs, coefs, S, tuple(fake.shape[2:])
+        return out_l1, out_c, out_s
 
     @staticmethod
-    def backward(ctx, g):
+    def backward(ctx, g_l1, g_c, g_s):
+        l1, content, style = ctx.want
         pairs = ctx.pairs
         dev = pairs[0][0].device
-        grads = [torch.empty_like(a) for a, _ in pairs]
-        terms = [_Term(a.data_ptr(), b.data_ptr(), ga.data_ptr(), a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
-                 for (a, b), ga, w in zip(pairs, grads, ctx.weights)]
-        gs = g.reshape(1).contiguous().float()
-        _lib.check(_lib.load().mg_loss_reduce_bwd(_device_table(terms, dev).data_ptr(), len(terms), gs.data_ptr(), ops._stream()),
-                   "mg_loss_reduce_bwd")
-        ctx.pairs = None
+        grads = [None] * len(pairs)
+        if l1:
+            grads = [torch.empty_like(a) for a, _ in pairs]
+            terms = [_Term(a.data_ptr(), b.data_ptr(), ga.data_ptr(), a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
+                     for (a, b), ga, w in zip(pairs, grads, ctx.weights)]
+            gs = g_l1.reshape(1).contiguous().float()
+            _lib.check(_lib.load().mg_loss_reduce_bwd(_device_table(terms, dev).data_ptr(), len(terms), gs.data_ptr(), ops._stream()),
+                       "mg_loss_reduce_bwd")
+        if content or style:
+            zero = torch.zeros((), device=dev, dtype=torch.float32)
+            g2 = torch.stack([g_s if style else zero, g_c if content else zero]).float().contiguous()
+            for i, (a, b) in enumerate(pairs):
+                coef = ctx.coefs[i] if style else None
+                ct = b if content and i == len(pairs) - 1 else None
+                if coef is None and ct is None:
+                    continue
+                grads[i] = ops.style_tap_grad(a, g2, coef=coef, content_t=ct, add=grads[i], out=grads[i])
+        ctx.pairs = ctx.coefs = None
         dimg = ctx.vgg.backward(ctx.S, grads, ctx.hw)
         ctx.S = None
-        return None, None, dimg, None
+        return None, None, None, dimg, None, None
+
+
+def _same_image(a, b):
+    return a is b or (a.shape == b.shape and bool(torch.equal(a, b)))
+
+
+def vgg_objective(vgg, fake, tag, style_image=None, l1=False, content=False, style=False, weights=VGG_WEIGHTS):
+    """(l1, content, style) of fake against tag (and the style image) from one VGG19 pass (_VGGObjectiveFn); None for a term not
+    asked for.  A style image equal to the tag (paired training loads the same file for both) is not run through VGG19 again:
+    the style targets then come from the tag half."""
+    if style:
+        err = style_min_size_error(*fake.shape[2:])
+        if err is not None:
+            raise err
+        if style_image is None or _same_image(style_image, tag):
+            style_image = None
+        else:
+            if style_image.shape != fake.shape:
+                raise ValueError("StyleContentLoss: fake %s and style image %s differ in shape" % (tuple(fake.shape), tuple(style_image.shape)))
+            style_image = style_image.float()
+    if fake.shape != tag.shape:
+        raise ValueError("VGG loss: fake %s and target %s differ in shape" % (tuple(fake.shape), tuple(tag.shape)))
+    dev = fake.device
+    if next(vgg.parameters()).device != dev:
+        vgg.to(dev)
+    return _VGGObjectiveFn.apply(vgg, weights, (bool(l1), bool(content), bool(style)), fake, tag.float(), style_image)
 
 
 class VGGLoss(nn.Module):
@@ -264,16 +342,68 @@ class VGGLoss(nn.Module):
             raise NotImplementedError("michigan_b200: --remove_background is not implemented")
         from .architecture import VGG19
         self.vgg = VGG19(state_dict=state_dict)
-        self.weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
+        self.weights = list(VGG_WEIGHTS)
         self.opt = opt
 
     def forward(self, x, y, label=None):
-        dev = x.device
-        if next(self.vgg.parameters()).device != dev:
-            self.vgg.to(dev)
-        if x.shape != y.shape:
-            raise ValueError("VGGLoss: fake %s and real %s differ in shape" % (tuple(x.shape), tuple(y.shape)))
-        return _VGGLossFn.apply(self.vgg, self.weights, x, y.float())
+        return vgg_objective(self.vgg, x, y, l1=True, weights=self.weights)[0]
+
+
+class StyleContentLoss(nn.Module):
+    """loss.py:656-711 (remove_background=False): (loss_c, loss_s) = forward(fake_image, style_image, content_image), with
+    loss_c = MSE(relu5_1(fake), relu5_1(content).detach()) and loss_s = sum over the five taps of MSE(mu_fake, mu_style) +
+    MSE(sigma_fake, sigma_style) (calc_mean_std: per (n, c), unbiased variance + 1e-5).  One VGG19 pass over fake || content
+    (|| style, unless it equals content) and one backward (_VGGObjectiveFn).  `vgg` shares another loss's VGG19 instance."""
+
+    def __init__(self, opt=None, vgg=None, state_dict=None):
+        super().__init__()
+        if getattr(opt, "remove_background", False):
+            raise NotImplementedError("michigan_b200: --remove_background is not implemented (calc_mean_std_mask / masked content loss)")
+        if vgg is None:
+            from .architecture import VGG19
+            vgg = VGG19(state_dict=state_dict)
+        self.vgg = vgg
+        self.opt = opt
+
+    def forward(self, fake_image, style_image, content_image, style_label=None, content_label=None):
+        _, loss_c, loss_s = vgg_objective(self.vgg, fake_image, content_image, style_image, content=True, style=True)
+        return loss_c, loss_s
+
+
+class _PixelL1Fn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, fake, tag, mask):
+        f, t = fake.detach().contiguous(), tag.detach().contiguous()
+        m = mask.detach().contiguous() if mask is not None else None
+        sums = ops.pixel_l1_fwd(f, t, m)
+        ctx.save_for_backward(f, t, m)
+        ctx.count = f.numel()
+        return (sums / ctx.count).float().reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        f, t, m = ctx.saved_tensors
+        gscale = (g.float() / ctx.count).reshape(1).contiguous()     # mean's backward: the fp32 gradient over the element count
+        return ops.pixel_l1_bwd(f, t, gscale, m), None, None
+
+
+class RGBBackgroundL1Loss(nn.Module):
+    """loss.py:388-400: L1(fake * m, image_tag.detach() * m), m = input_semantics[:, 0] (the background channel of the one-hot
+    label), one kernel each way (mg_pixel_l1_fwd / _bwd)."""
+
+    def forward(self, fake, input_semantics, image_tag):
+        if fake.shape != image_tag.shape or fake.shape[1] != 3:
+            raise ValueError("RGBBackgroundL1Loss: expected two [N,3,H,W] images, got %s and %s" % (tuple(fake.shape), tuple(image_tag.shape)))
+        return _PixelL1Fn.apply(fake, image_tag.float(), input_semantics[:, 0].float())
+
+
+class RGBL1Loss(nn.Module):
+    """The rgb term, nn.L1Loss()(fake, image_tag.detach()) (pix2pix_model.py:51, 328-333), on mg_pixel_l1_fwd / _bwd."""
+
+    def forward(self, fake, image_tag):
+        if fake.shape != image_tag.shape or fake.shape[1] != 3:
+            raise ValueError("RGBL1Loss: expected two [N,3,H,W] images, got %s and %s" % (tuple(fake.shape), tuple(image_tag.shape)))
+        return _PixelL1Fn.apply(fake, image_tag.float(), None)
 
 
 class _LabLossFn(torch.autograd.Function):

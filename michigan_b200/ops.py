@@ -696,6 +696,70 @@ def lab_loss_bwd(fake, real, gscale):
     return dfake
 
 
+class StyleTap(C.Structure):
+    """One record of mg_style_loss_fwd's host table (include/michigan_b200.h)."""
+    _fields_ = [("sums_f", C.c_void_p), ("sums_t", C.c_void_p), ("coef", C.c_void_p), ("M", C.c_longlong), ("N", C.c_int32),
+                ("C", C.c_int32)]
+
+
+def channel_sums(x):
+    """Per-(image, channel) fp64 sums of an NHWC fp32 tensor -> [N, 2, C] (sum x, sum x^2), mg_in_stats."""
+    _chk(x, "x")
+    N, H, W, Cc = x.shape
+    sums = torch.zeros((N, 2, Cc), device=x.device, dtype=torch.float64)
+    check(_lib.load().mg_in_stats(_p(x), N, H * W, Cc, _p(sums), _stream()), "mg_in_stats")
+    return sums
+
+
+def style_loss_fwd(taps):
+    """taps: list of (sums_fake [N,2,C], sums_target [N,2,C], M) -> ([1] float64 loss sum over the taps, [coef [N,3,C] per tap]).
+    One mg_style_loss_fwd launch for every tap."""
+    recs, coefs = [], []
+    for sf, st, M in taps:
+        _chk(sf, "sums_f", torch.float64); _chk(st, "sums_t", torch.float64)
+        N, _, Cc = sf.shape
+        assert st.shape == sf.shape, (st.shape, sf.shape)
+        coef = torch.empty((N, 3, Cc), device=sf.device, dtype=torch.float32)
+        coefs.append(coef)
+        recs.append(StyleTap(_p(sf), _p(st), _p(coef), int(M), N, Cc))
+    loss = torch.zeros(1, device=taps[0][0].device, dtype=torch.float64)
+    table = (StyleTap * len(recs))(*recs)
+    check(_lib.load().mg_style_loss_fwd(C.cast(table, C.c_void_p), len(recs), _p(loss), _stream()), "mg_style_loss_fwd")
+    return loss, coefs
+
+
+def style_tap_grad(x, g, coef=None, content_t=None, add=None, out=None):
+    """Gradient w.r.t. the fake tap x [N,h,w,C] of g[0] * style loss (coef from style_loss_fwd) + g[1] * content loss (MSE against
+    content_t); g: [2] fp32 device tensor.  add (may be `out`) is accumulated; out defaults to a new tensor."""
+    _chk(x, "x"); _chk(g, "g"); _chk(coef, "coef"); _chk(content_t, "content_t"); _chk(add, "add"); _chk(out, "out")
+    N, H, W, Cc = x.shape
+    if out is None:
+        out = torch.empty_like(x)
+    check(_lib.load().mg_style_tap_grad(_p(x), _p(coef), _p(content_t), _p(add), _p(out), _p(g), N, H * W, Cc, _stream()),
+          "mg_style_tap_grad")
+    return out
+
+
+def pixel_l1_fwd(fake, tag, mask=None):
+    """-> [1] float64 device tensor: sum |m*fake - m*tag| over [N,3,H,W] (mask [N,H,W] broadcast over channels; None = 1)."""
+    _chk(fake, "fake"); _chk(tag, "tag"); _chk(mask, "mask")
+    N, _, H, W = fake.shape
+    assert fake.shape == tag.shape and fake.shape[1] == 3, (fake.shape, tag.shape)
+    assert mask is None or tuple(mask.shape) == (N, H, W), mask.shape
+    sums = torch.zeros(1, device=fake.device, dtype=torch.float64)
+    check(_lib.load().mg_pixel_l1_fwd(_p(fake), _p(tag), _p(mask), _p(sums), N, H, W, _stream()), "mg_pixel_l1_fwd")
+    return sums
+
+
+def pixel_l1_bwd(fake, tag, gscale, mask=None):
+    """d fake [N,3,H,W] of gscale[0] * pixel_l1_fwd(fake, tag, mask); gscale: [1] fp32 device tensor."""
+    _chk(fake, "fake"); _chk(tag, "tag"); _chk(gscale, "gscale"); _chk(mask, "mask")
+    N, _, H, W = fake.shape
+    dfake = torch.empty_like(fake)
+    check(_lib.load().mg_pixel_l1_bwd(_p(fake), _p(tag), _p(mask), _p(gscale), _p(dfake), N, H, W, _stream()), "mg_pixel_l1_bwd")
+    return dfake
+
+
 def instance_norm_act_fwd(x, act=ACT_LRELU, eps=1e-5, round_out=False, pmul=None, out16=None):
     """Training variant of instance_norm_act: also returns the (rstd, shift) table needed by in_bwd.
     -> (y, ss), or (y, ss, hi, lo|None) with out16=(fmt, want_lo) (16-bit operand copies for the next tensor-core conv)."""

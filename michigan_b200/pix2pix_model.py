@@ -2,8 +2,9 @@
 models/pix2pix_model.py (forward 62-122, create_optimizers 124-152, preprocess_input 209-254,
 compute_generator_loss 257-365, compute_discriminator_loss 367-398, generate_fake 505-541,
 discriminate 546-594) for the in-scope configuration: netG=spadeb, netD=multiscale, hinge GAN loss +
-GAN feature loss, optionally the VGG perceptual, Lab colour and Gabor orientation losses of the README's training command.  With the reference checkout present, `michigan_b200.install()` lets the reference's
-own Pix2PixModel/Pix2PixTrainer drive these networks instead (INTEGRATION.md); this class is the
+GAN feature loss and, each behind its --no_* flag, every other term of the reference's curr_step-1 objective (VGG
+perceptual, style / content, background and rgb L1, Lab colour, Gabor orientation / confidence).  With the reference checkout
+present, `michigan_b200.install()` lets the reference's own Pix2PixModel/Pix2PixTrainer drive these networks instead (INTEGRATION.md); this class is the
 stand-alone equivalent used by bench.py and the tests on machines without the reference.
 """
 import os
@@ -12,7 +13,8 @@ import torch
 import torch.nn.functional as F
 
 from . import networks, ops
-from .networks.loss import GANFeatLoss, GANLoss, LabColorLoss, VGGLoss
+from .networks.loss import (GANFeatLoss, GANLoss, LabColorLoss, RGBBackgroundL1Loss, RGBL1Loss, StyleContentLoss, VGGLoss,
+                            vgg_objective)
 
 
 class Pix2PixModel(torch.nn.Module):
@@ -29,19 +31,9 @@ class Pix2PixModel(torch.nn.Module):
         for flag in ("use_vae", "use_blender", "use_instance_feat", "unpairTrain"):
             if getattr(opt, flag, False):
                 raise NotImplementedError("michigan_b200: --%s is outside the hot path (SURVEY.md §8)" % flag)
-        if opt.isTrain:
-            # The reference's generator objective also contains VGG / style / content / background / rgb / lab / orientation
-            # terms, all ON by default (pix2pix_model.py:296-345).  This stand-alone model implements the SURVEY §8d loss set
-            # (hinge GAN + GAN feature matching), the VGG perceptual and Lab colour losses of the README's training command
-            # (--no_vgg_loss / --no_lab_loss to drop them) and the Gabor orientation / confidence loss (loss.py:274-385,
-            # --no_orient_loss): anything else must be switched off explicitly rather than silently dropped.
-            # (Through michigan_b200.install() the reference's own Pix2PixModel computes whatever losses it is asked for.)
-            missing = [f for f in ("no_style_loss", "no_content_loss", "no_background_loss", "no_rgb_loss")
-                       if not getattr(opt, f, False)]
-            if missing:
-                raise NotImplementedError("michigan_b200.Pix2PixModel trains with the hinge GAN, GAN_Feat, VGG, Lab and orientation "
-                                          "losses only; pass --%s (or drive the reference's Pix2PixModel through "
-                                          "michigan_b200.install())" % " --".join(missing))
+        # Every term of the reference's generator objective for curr_step 1 (pix2pix_model.py:296-345) is computed here: hinge
+        # GAN, GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT, CONFIDENCE, each dropped by its --no_* flag.
+        # --remove_background and --balance_Lab are refused by the loss classes.
         self.netIG = None
         if getattr(opt, "use_ig", False):
             self.netIG = networks.define_IG(opt)
@@ -53,6 +45,14 @@ class Pix2PixModel(torch.nn.Module):
             self.criterionGANFeat = GANFeatLoss(opt)
             if not getattr(opt, "no_vgg_loss", False):
                 self.criterionVGG = VGGLoss(opt)
+            if not (getattr(opt, "no_style_loss", False) and getattr(opt, "no_content_loss", False)):
+                # one VGG19 instance for the perceptual and the style / content losses (they share one pass, _vgg_terms)
+                shared = self.criterionVGG.vgg if hasattr(self, "criterionVGG") else None
+                self.criterionStyleContent = StyleContentLoss(opt, vgg=shared)
+            if not getattr(opt, "no_background_loss", False):
+                self.criterionBackground = RGBBackgroundL1Loss()
+            if not getattr(opt, "no_rgb_loss", False):
+                self.criterionRGBL1 = RGBL1Loss()
             if not getattr(opt, "no_lab_loss", False):
                 self.criterionLabL1 = LabColorLoss(opt)
             if not getattr(opt, "no_orient_loss", False):
@@ -197,9 +197,20 @@ class Pix2PixModel(torch.nn.Module):
         ref_is_tag = bool(torch.sum(input_tag[:, 1] - input_ref[:, 1]) == 0)
         if self.opt.curr_step == 1 and not self.opt.no_ganFeat_loss and ref_is_tag:
             G_losses["GAN_Feat"] = self.criterionGANFeat(pred_fake, pred_real, label_tag)
-        # pix2pix_model.py:300-307 and 335-340: in the reference's key order (GAN, GAN_Feat, VGG, lab, ORIENT, CONFIDENCE)
-        if self.opt.curr_step == 1 and not getattr(self.opt, "no_vgg_loss", False) and ref_is_tag:
-            G_losses["VGG"] = self.criterionVGG(fake_image, image_tag, label_tag) * self.opt.lambda_vgg
+        # pix2pix_model.py:300-340, in the reference's key order (GAN, GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT,
+        # CONFIDENCE): VGG, background, rgb and lab only when ref is tag, content and style whenever curr_step is 1
+        if self.opt.curr_step == 1:
+            vgg, content, style = self._vgg_terms(fake_image, image_ref, image_tag, ref_is_tag)
+            if vgg is not None:
+                G_losses["VGG"] = vgg * self.opt.lambda_vgg
+            if content is not None:
+                G_losses["content"] = content * self.opt.lambda_content
+            if style is not None:
+                G_losses["style"] = style * self.opt.lambda_style
+        if self.opt.curr_step == 1 and not getattr(self.opt, "no_background_loss", False) and ref_is_tag:
+            G_losses["background"] = self.criterionBackground(fake_image, input_tag, image_tag) * self.opt.lambda_background
+        if self.opt.curr_step == 1 and not getattr(self.opt, "no_rgb_loss", False) and ref_is_tag:
+            G_losses["rgb"] = self.criterionRGBL1(fake_image, image_tag.detach()) * self.opt.lambda_rgb
         if self.opt.curr_step == 1 and not getattr(self.opt, "no_lab_loss", False) and ref_is_tag:
             G_losses["lab"] = self.criterionLabL1(fake_image, image_tag.detach(), label_tag) * self.opt.lambda_lab
         if not getattr(self.opt, "no_orient_loss", False):
@@ -209,6 +220,18 @@ class Pix2PixModel(torch.nn.Module):
             if not getattr(self.opt, "no_confidence_loss", False):
                 G_losses["CONFIDENCE"] = confidence_loss * self.opt.lambda_confidence
         return G_losses, fake_image
+
+    def _vgg_terms(self, fake_image, image_ref, image_tag, ref_is_tag):
+        """(VGG, content, style), None for a term that is off: one VGG19 pass over fake || tag (|| ref, unless it equals tag) for
+        all of them (networks.loss.vgg_objective); VGG alone goes through criterionVGG, as before."""
+        l1 = not getattr(self.opt, "no_vgg_loss", False) and ref_is_tag
+        content = not getattr(self.opt, "no_content_loss", False)
+        style = not getattr(self.opt, "no_style_loss", False)
+        if not (content or style):
+            return (self.criterionVGG(fake_image, image_tag) if l1 else None), None, None
+        crit = self.criterionStyleContent
+        return vgg_objective(crit.vgg, fake_image, image_tag, image_ref, l1=l1, content=content, style=style,
+                             weights=self.criterionVGG.weights if l1 else None)
 
     def compute_discriminator_loss(self, input_ref, input_tag, image_ref, image_tag, orient_mask, noise):
         with torch.no_grad():

@@ -1,10 +1,11 @@
 """Per-kernel GPU time of one generator-forward step and one train step at the benchmark configuration (batch 8, 512x512,
 synthetic inputs, random-init weights), from torch.profiler CUDA activity.
 
-    python tools/kernel_times.py OUT_DIR [--batch N] [--warmup W] [--objective readme]
+    python tools/kernel_times.py OUT_DIR [--batch N] [--warmup W] [--objective readme|default]
 
 --objective readme trains with the loss set of the README's training command (hinge GAN, GAN_Feat, VGG, lab, ORIENT; seeded
-stand-in VGG19 weights) and adds a "train step, paper objective" table.  Writes OUT_DIR/kernel_times.md (one table per workload: kernel, launches, total ms, share of the step's kernel time) and
+stand-in VGG19 weights) and adds a "train step, paper objective" table; --objective default trains with the reference's default
+loss set (also content, style, background, rgb, CONFIDENCE) and adds a "train step, default objective" table.  Writes OUT_DIR/kernel_times.md (one table per workload: kernel, launches, total ms, share of the step's kernel time) and
 OUT_DIR/kernel_times.json.  Templated kernels are listed per instantiation, so the variant of each conv kernel is visible.
 Selects the library like everything else (MICHIGAN_B200_LIB), which makes before/after tables of two builds comparable.
 """
@@ -21,6 +22,11 @@ SIZE = 512
 
 
 README_LOSSES = dict(no_vgg_loss=False, no_lab_loss=False, no_orient_loss=False)
+# the reference's default generator objective (options/train_options.py: every no_* off): README_LOSSES + content, style,
+# background, rgb and the confidence loss
+DEFAULT_LOSSES = dict(README_LOSSES, no_style_loss=False, no_content_loss=False, no_background_loss=False, no_rgb_loss=False,
+                      no_confidence_loss=False)
+OBJECTIVES = {"readme": ("train step, paper objective", README_LOSSES), "default": ("train step, default objective", DEFAULT_LOSSES)}
 
 
 def build_model(batch, **losses):
@@ -80,7 +86,7 @@ def main():
     ap.add_argument("out_dir")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--objective", choices=["8d", "readme"], default="8d")
+    ap.add_argument("--objective", choices=["8d", "readme", "default"], default="8d")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("kernel_times.py needs a CUDA device")
@@ -99,12 +105,13 @@ def main():
     wrap = DataParallelWithCallback(model, device_ids=[0])
     optG, optD = model.create_optimizers(model.opt)
     tables["train step"] = kernel_table(lambda: train_iteration(wrap, optG, optD, dict(dev)), a.warmup)
-    if a.objective == "readme":
+    if a.objective in OBJECTIVES:
+        title, losses = OBJECTIVES[a.objective]
         del wrap, optG, optD, model
-        model = build_model(a.batch, **README_LOSSES)
+        model = build_model(a.batch, **losses)
         wrap = DataParallelWithCallback(model, device_ids=[0])
         optG, optD = model.create_optimizers(model.opt)
-        tables["train step, paper objective"] = kernel_table(lambda: train_iteration(wrap, optG, optD, dict(dev)), a.warmup)
+        tables[title] = kernel_table(lambda: train_iteration(wrap, optG, optD, dict(dev)), a.warmup)
 
     os.makedirs(a.out_dir, exist_ok=True)
     gpu = torch.cuda.get_device_name(0)

@@ -1,6 +1,9 @@
-"""Cost of the paper's objective: the train step with the README's loss set (hinge GAN, GAN_Feat, VGG, lab, ORIENT) against the
-SURVEY §8d set (hinge GAN, GAN_Feat), alternated in one process, plus the VGG and Lab loss kernels on their own and, for
-context, the oracle's VGG restatement run eagerly on CUDA (cuDNN) with the same seeded weights.
+"""Cost of the paper's objective: the train step with the README's loss set (hinge GAN, GAN_Feat, VGG, lab, ORIENT) and with the
+reference's default loss set (also content, style, background, rgb, CONFIDENCE) against the SURVEY §8d set (hinge GAN, GAN_Feat),
+alternated in one process, plus the VGG and Lab loss kernels on their own and, for context, the oracle's VGG restatement run
+eagerly on CUDA (cuDNN) with the same seeded weights.  The VGG terms of the default objective are timed as one combined pass
+(VGG L1 + content + style, ref == tag and ref != tag) and as VGGLoss + StyleContentLoss called separately (what the reference's
+Pix2PixModel does under install()), with the style statistics and tap-gradient kernels on their own.
 
     python tools/vgg_lab_time.py OUT_DIR [--batch 8] [--steps 5] [--rounds 3]
 
@@ -69,8 +72,10 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("vgg_lab_time.py needs a CUDA device")
     import oracle_vgg_lab as ovl
-    from kernel_times import README_LOSSES, build_model
-    from michigan_b200.networks import LabColorLoss, VGGLoss
+    from kernel_times import DEFAULT_LOSSES, README_LOSSES, build_model
+    from michigan_b200 import ops
+    from michigan_b200.networks import LabColorLoss, StyleContentLoss, VGGLoss
+    from michigan_b200.networks.loss import vgg_objective
     from michigan_b200.networks.sync_batchnorm import DataParallelWithCallback
     from michigan_b200.options import make_opt
     from michigan_b200.pix2pix_model import train_iteration
@@ -82,7 +87,7 @@ def main():
     data = synthetic_batch(n, SIZE, 1234)
     dev = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in data.items()}
     legs = {}
-    for name, losses in (("8d", {}), ("readme", README_LOSSES)):
+    for name, losses in (("8d", {}), ("readme", README_LOSSES), ("default", DEFAULT_LOSSES)):
         model = build_model(n, **losses)
         wrap = DataParallelWithCallback(model, device_ids=[0])
         optG, optD = model.create_optimizers(model.opt)
@@ -120,6 +125,44 @@ def main():
     ms_o = timed(vgg_oracle, 5)
     res["vgg_cudnn_ms"] = ms_o
     print("VGG loss fwd+bwd (oracle, eager cuDNN, torch defaults): %.2f ms, %.0f TFLOP/s algorithmic" % (ms_o, flop / ms_o / 1e9))
+
+    # the VGG terms of the default objective: one combined pass against the two loss classes called separately
+    sc = StyleContentLoss(make_opt(), vgg=crit.vgg)
+    ref = (torch.rand(n, 3, SIZE, SIZE, generator=g) * 2 - 1).cuda()
+
+    def separate():
+        x = fake.detach().requires_grad_()
+        lc, ls = sc(x, real, real)
+        (crit(x, real) + lc + ls).backward()
+
+    def combined(style):
+        x = fake.detach().requires_grad_()
+        sum(vgg_objective(crit.vgg, x, real, style, l1=True, content=True, style=True)).backward()
+
+    for r in range(a.rounds):
+        for key, fn in (("separate", separate), ("combined", lambda: combined(real)), ("combined_ref_ne_tag", lambda: combined(ref))):
+            ms = timed(fn, 5)
+            res.setdefault("vgg_default_%s_ms" % key, []).append(ms)
+            print("round %d  VGG + content + style fwd+bwd, %-20s %.2f ms" % (r, key, ms))
+    taps, _ = crit.vgg.run(ops.nchw_to_nhwc(torch.cat([fake, real]).contiguous(), 4))
+    gv = torch.ones(2, device="cuda")
+    state = {}
+
+    def style_fwd():
+        sums = [ops.channel_sums(t) for t in taps]
+        state["coefs"] = ops.style_loss_fwd([(s[:n], s[n:], t.shape[1] * t.shape[2]) for s, t in zip(sums, taps)])[1]
+
+    def style_bwd():
+        for i, t in enumerate(taps):
+            ops.style_tap_grad(t[:n], gv, coef=state["coefs"][i], content_t=t[n:] if i == 4 else None)
+
+    tap_bytes = sum(t.numel() * 4 for t in taps)
+    ms_f, ms_b = timed(style_fwd, 20), timed(style_bwd, 20)
+    res["style_stats_ms"], res["style_tap_grad_ms"] = ms_f, ms_b
+    print("style statistics + loss (5 x mg_in_stats + mg_style_loss_fwd, %.2f GB of taps read): %.3f ms, %.0f GB/s"
+          % (tap_bytes / 1e9, ms_f, tap_bytes / ms_f / 1e6))
+    print("style tap gradients (5 x mg_style_tap_grad, fake half read + written, relu5_1 target read): %.3f ms, %.0f GB/s"
+          % (ms_b, (tap_bytes + taps[4].numel() * 2) / ms_b / 1e6))
 
     lab = LabColorLoss(make_opt())
 
