@@ -98,7 +98,8 @@ typedef struct mg_igemm_args {
      * then 16-bit arrays, Cin % 64 == 0).  split != 0: three-pass split precision A_hi*W_hi + A_lo*W_hi +
      * A_hi*W_lo with in = A_hi, in_lo = A_lo and wpack = [CoutG][tap][hi|lo][Cin] (mg_pack_weight16).
      * out_hi / out_lo: optional 16-bit copies of the result (hi = cvt(y), lo = cvt(y - hi)), fmt out16_fmt;
-     * `out` may then be null. */
+     * `out` may then be null.  fp16 hi is clamped to +-65504 first; lo is not, so it is +-inf where
+     * |y - hi| >= 65520 (|y| above about 131008): fp16 hi/lo pairs carry |y| < 131008 only. */
     const void* in_lo;
     int32_t a_fmt, split;
     void* out_hi;
