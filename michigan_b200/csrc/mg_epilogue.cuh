@@ -311,13 +311,69 @@ __device__ __forceinline__ void epi_store_pair(const IgemmParams& p, size_t pix,
     }
 }
 
+// The same for the SPADE epilogue of epilogue_frag: rounding, fp32 store (or accumulation) when `store`, and the packed 16-bit
+// hi/lo words, which epi_store16_quad writes.
+template <int SPEC>
+__device__ __forceinline__ void epi_finish_pair(const IgemmParams& p, size_t pix, int ch, bool store, float y0, float y1, uint32_t& hi,
+                                                uint32_t& lo) {
+    constexpr bool kS = SPEC == 1 || SPEC == 2;
+    if (!kS && p.round_out != 0) { y0 = round_tf32(y0); y1 = round_tf32(y1); }
+    if (!kS && p.out != nullptr && store) {
+        float2* op = reinterpret_cast<float2*>(p.out + pix * p.Cout + ch);
+        if (p.accumulate) {
+            const float2 o = *op;
+            y0 += o.x; y1 += o.y;
+        }
+        *op = make_float2(y0, y1);
+    }
+    if (kS || p.out_hi != nullptr) epi_split16(y0, y1, kS ? 2 : p.out16_fmt, hi, lo);
+}
+
+// 4 x 4 transposition of 32-bit words across the lanes of a quad (two butterfly steps): lane q's w[i] becomes lane i's w[q].
+// Every lane of the warp must take part.
+__device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int lane) {
+    const bool b1 = (lane & 2) != 0, b0 = (lane & 1) != 0;
+    uint32_t s0 = b1 ? w[0] : w[2], s1 = b1 ? w[1] : w[3];
+    s0 = __shfl_xor_sync(0xffffffffu, s0, 2);
+    s1 = __shfl_xor_sync(0xffffffffu, s1, 2);
+    if (b1) { w[0] = s0; w[1] = s1; } else { w[2] = s0; w[3] = s1; }
+    s0 = b0 ? w[0] : w[1];
+    s1 = b0 ? w[2] : w[3];
+    s0 = __shfl_xor_sync(0xffffffffu, s0, 1);
+    s1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+    if (b0) { w[0] = s0; w[2] = s1; } else { w[1] = s0; w[3] = s1; }
+}
+
+// The 16-bit copies of four 8-channel blocks of one pixel: hi[i] / lo[i] hold this lane's pair 2 (lane & 3) of block i, whose
+// first channel is cb + 8 i.  After a quad transposition lane q holds all four pairs of block q and writes them with one 16-byte
+// store, so a quad writes 64 contiguous bytes (whole 32-byte sectors) instead of four lanes x 4 bytes per block.  Every lane
+// of the warp must call it; `store` masks the pixel.  Cout is a multiple of 32 (every N tile is full), so a block is either
+// wholly inside the output or wholly outside, and pix * Cout * 2 bytes is 16-byte aligned.
+template <int SPEC>
+__device__ __forceinline__ void epi_store16_quad(const IgemmParams& p, size_t pix, int cb, bool store, uint32_t (&hi)[4],
+                                                 uint32_t (&lo)[4], int lane) {
+    constexpr bool kS = SPEC == 1 || SPEC == 2;
+    if (!kS && p.out_hi == nullptr) return;
+    const bool has_lo = kS || p.out_lo != nullptr;
+    quad_transpose(hi, lane);
+    if (has_lo) quad_transpose(lo, lane);
+    const int ch = cb + 8 * (lane & 3);
+    if (!store || ch >= p.Cout || ((MG_DBGV(p) & (8 | 32)) && hi[0] != 12345u)) return;
+    const size_t eo = pix * p.Cout + ch;
+    *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out_hi) + eo) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    if (has_lo) *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out_lo) + eo) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
+
 // The two finished M tiles of a conv3x3_group_kernel group (TW = 8, TH = 16, TN = 1) straight from the wgmma accumulators:
 // no shared-memory tile, no transposition, no barrier.  Thread (warpgroup wg, warp quarter = warp & 3, lane) holds in acc_t
 // rows 64 wg + 16 quarter + lane/4 + 8h (h = 0, 1) of M tile t, i.e. pixel (ow = 8 (tw0 + t) + lane/4, oh = 16 th + 8 wg +
 // 2 quarter + h), and in register 4j + 2h + e the accumulator column 8j + 2 (lane & 3) + e.  So every thread owns 4 pixels and
 // a fixed set of channel pairs, and what the epilogue combines is in the same thread: SPADE's gamma and beta (columns c and
 // c + BN/2) and the two halves of merged split precision (c and c + BN).  The per-pixel side inputs of a tile (SPADE x or the
-// residual, blend maps, pscale / pmul) are loaded before its arithmetic; the per-channel parameters are read through L1.
+// residual, blend maps, pscale / pmul) are loaded before its arithmetic; the per-channel parameters are read through L1 (both
+// tiles' accumulators and x leave no registers to keep them for the whole group).  SPADE's 16-bit copies are transposed
+// across each quad and written 16 bytes per lane (epi_store16_quad).  The plain epilogue keeps 4-byte 16-bit stores: the
+// transposition's words do not fit next to its side inputs at merged BN = 64 without spills.
 // Same arithmetic as epilogue_tile (the epi_* helpers), so every element gets the same bits.
 template <int SPEC, int BN, bool MERGED, int R>
 __device__ __forceinline__ void epilogue_frag(const IgemmParams& p, const float (&acc0)[R], const float (&acc1)[R], int nt, int tw0,
@@ -360,43 +416,57 @@ __device__ __forceinline__ void epilogue_frag(const IgemmParams& p, const float 
                                           ? __ldg(reinterpret_cast<const float2*>(p.x + src[t][h] * p.Cout + ch0 + 8 * j))
                                           : make_float2(0.f, 0.f);
             };
-            auto tile = [&](const float (&acc)[R], auto tc) {
+            // blocks of four column groups j (32 channels): the 16-bit words of a block leave through epi_store16_quad, so the
+            // arithmetic runs for masked pixels too (their loads and stores are skipped) and every lane reaches the shuffles
+            auto block = [&](const float (&acc)[R], auto tc, int k) {
                 constexpr int t = decltype(tc)::value;
+                {
+                    uint32_t hi[2][4], lo[2][4];
 #pragma unroll
-                for (int j = 0; j < J; ++j) {
-                    const int ch = ch0 + 8 * j;
-                    if (ch >= p.Cout) continue;
-                    const float2 sc = __ldg(reinterpret_cast<const float2*>(p.nscale + ch));
-                    const float2 sh = __ldg(reinterpret_cast<const float2*>(p.nshift + ch));
-                    const float2 g1 = __ldg(reinterpret_cast<const float2*>(p.gbias1 + ch));
-                    const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bbias + ch));
+                    for (int i = 0; i < 4; ++i) {
+                        const int j = 4 * k + i, ch = ch0 + 8 * j;
+                        const bool cok = ch < p.Cout;
+                        const float2 z = make_float2(0.f, 0.f);
+                        const float2 sc = cok ? __ldg(reinterpret_cast<const float2*>(p.nscale + ch)) : z;
+                        const float2 sh = cok ? __ldg(reinterpret_cast<const float2*>(p.nshift + ch)) : z;
+                        const float2 g1 = cok ? __ldg(reinterpret_cast<const float2*>(p.gbias1 + ch)) : z;
+                        const float2 bb = cok ? __ldg(reinterpret_cast<const float2*>(p.bbias + ch)) : z;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (!ok[t][h]) continue;
-                        const float2 x = side_ok ? xv[t][h][j] : sc;
-                        float g[2], b[2], gs[2], y[2];
+                        for (int h = 0; h < 2; ++h) {
+                            const bool st = ok[t][h] && cok;
+                            const float2 x = side_ok ? xv[t][h][j] : sc;
+                            float g[2], b[2], gs[2], y[2];
 #pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            g[e] = acc[4 * j + 2 * h + e];
-                            b[e] = acc[4 * (j + kBeta) + 2 * h + e];
-                            if (MERGED) {
-                                g[e] += acc[4 * (j + kLo) + 2 * h + e];
-                                b[e] += acc[4 * (j + kBeta + kLo) + 2 * h + e];
+                            for (int e = 0; e < 2; ++e) {
+                                g[e] = acc[4 * j + 2 * h + e];
+                                b[e] = acc[4 * (j + kBeta) + 2 * h + e];
+                                if (MERGED) {
+                                    g[e] += acc[4 * (j + kLo) + 2 * h + e];
+                                    b[e] += acc[4 * (j + kBeta + kLo) + 2 * h + e];
+                                }
                             }
+                            y[0] = epi_spade_out(epi_spade_mod(x.x, sc.x, sh.x, g1.x, g[0], gs[0]), bb.x, b[0], act);
+                            y[1] = epi_spade_out(epi_spade_mod(x.y, sc.y, sh.y, g1.y, g[1], gs[1]), bb.y, b[1], act);
+                            if (has_aux && st) *reinterpret_cast<float2*>(p.aux + pix[t][h] * p.Cout + ch) = make_float2(gs[0], gs[1]);
+                            epi_finish_pair<SPEC>(p, pix[t][h], ch, st, y[0], y[1], hi[h][i], lo[h][i]);
                         }
-                        y[0] = epi_spade_out(epi_spade_mod(x.x, sc.x, sh.x, g1.x, g[0], gs[0]), bb.x, b[0], act);
-                        y[1] = epi_spade_out(epi_spade_mod(x.y, sc.y, sh.y, g1.y, g[1], gs[1]), bb.y, b[1], act);
-                        if (has_aux) *reinterpret_cast<float2*>(p.aux + pix[t][h] * p.Cout + ch) = make_float2(gs[0], gs[1]);
-                        epi_store_pair<SPEC>(p, pix[t][h], ch, y[0], y[1]);
                     }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) epi_store16_quad<SPEC>(p, pix[t][h], ch0 - c0 + 32 * k, ok[t][h], hi[h], lo[h], lane);
                 }
             };
-            // SPEC 1/2 have the registers to fetch tile 1's x before tile 0's arithmetic; the generic variant fetches it after
-            load_x(std::integral_constant<int, 0>{});
-            if constexpr (kS) load_x(std::integral_constant<int, 1>{});
-            tile(acc0, std::integral_constant<int, 0>{});
-            if constexpr (!kS) load_x(std::integral_constant<int, 1>{});
-            tile(acc1, std::integral_constant<int, 1>{});
+            // SPEC 1/2 fetch tile 1's x once tile 0's first block has freed its registers, so that its latency overlaps the
+            // rest of tile 0; the generic variant fetches it after tile 0
+            using T0 = std::integral_constant<int, 0>;
+            using T1 = std::integral_constant<int, 1>;
+            load_x(T0{});
+            block(acc0, T0{}, 0);
+            if constexpr (kS) load_x(T1{});
+#pragma unroll
+            for (int k = 1; k < J / 4; ++k) block(acc0, T0{}, k);
+            if constexpr (!kS) load_x(T1{});
+#pragma unroll
+            for (int k = 0; k < J / 4; ++k) block(acc1, T1{}, k);
             return;
         }
     }
