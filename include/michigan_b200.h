@@ -387,6 +387,21 @@ int mg_lab_loss_fwd(const float* fake_nchw, const float* real_nchw, double* sums
 int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, const float* gscale, float* dfake_nchw, int N, int H, int W,
                     void* stream);
 
+/* ---- hair-average Lab loss (models/networks/loss.py:534-621 HairAvgLabLoss, balance_Lab = False) -----------------------------
+ * Replaces rgb2xyz / xyz2lab of fake and real (loss.py:549-570, the same per-pixel Lab as mg_lab_loss_fwd, L = 116 f(Y) - 16 if
+ * Y > 0.008856 else 903.3 Y), cal_hair_avg (loss.py:571-577) and the L1 of the a, b averages (loss.py:601-621).
+ * fake, real [N,3,H,W] fp32 in [-1,1]; mask_fake, mask_real [N,1,H,W] fp32 (the tag's and the reference's hair).
+ * mg_hair_avg_lab_fwd: sums [N][2][4] fp64 (written, not accumulated) = per image {sum m L, sum m a, sum m b, sum m} of fake with
+ *   mask_fake, then of real with mask_real; each product rounded to fp32 first.  Partials are added in a fixed order: two runs
+ *   give the same bits.  avg = sum / (sum m, 0 -> 1); loss = mean over the N x 2 values |avg_f - avg_r| of a and b.
+ * mg_hair_avg_lab_bwd: dfake = mask_fake * (T[n][0] da/dfake + T[n][1] db/dfake), T[n][j] = gscale[0] / (2N) sgn(avg_f - avg_r)
+ *   / cnt_f formed on the device from `sums` (gscale: device float = upstream gradient); f' branch by branch as mg_lab_loss_bwd.
+ *   real is detached: there is no d real. */
+int mg_hair_avg_lab_fwd(const float* fake_nchw, const float* real_nchw, const float* mask_fake, const float* mask_real, double* sums,
+                        int N, int H, int W, void* stream);
+int mg_hair_avg_lab_bwd(const float* fake_nchw, const float* mask_fake, const double* sums, const float* gscale, float* dfake_nchw,
+                        int N, int H, int W, void* stream);
+
 /* ---- style and content losses (models/networks/loss.py:624-711 StyleContentLoss with remove_background = False) ----------
  * Replaces calc_mean_std (loss.py:624-632), calc_style_loss and calc_content_loss (loss.py:662-683) over the five VGG19 taps.
  * The per-(n, c) statistics are mg_in_stats' fp64 sums ([N][2][C]: sum x, sum x^2) of each fp32 NHWC tap, one call per tap over

@@ -127,6 +127,8 @@ SIGNATURES = {
     "mg_relu_bwd16": [_p, _p, _p, _p, _i, _p, _p, _ll, _p],
     "mg_lab_loss_fwd": [_p, _p, _p, _i, _i, _i, _p],
     "mg_lab_loss_bwd": [_p, _p, _p, _p, _i, _i, _i, _p],
+    "mg_hair_avg_lab_fwd": [_p, _p, _p, _p, _p, _i, _i, _i, _p],
+    "mg_hair_avg_lab_bwd": [_p, _p, _p, _p, _p, _i, _i, _i, _p],
     "mg_style_loss_fwd": [_p, _i, _p, _p],
     "mg_style_tap_bytes": [],
     "mg_style_tap_grad": [_p, _p, _p, _p, _p, _p, _i, _ll, _i, _p],

@@ -9,6 +9,7 @@
 //                         tensor the forward pooled, so both agree bit for bit; fp32 and/or bf16 (conv_dgrad's dy16) out;
 //   mg_relu_bwd16         ReLU backward of the layers without a pool, same outputs;
 //   mg_lab_loss_fwd/bwd   the Lab colour L1 loss over fake and real in one pass; d fake written directly (NCHW);
+//   mg_hair_avg_lab_fwd/bwd  HairAvgLabLoss (loss.py:534-621): masked per-image Lab sums of fake and real, and d fake;
 //   mg_style_loss_fwd     the style loss of StyleContentLoss (loss.py:624-711) for every tap in one launch, from mg_in_stats' sums;
 //   mg_style_tap_grad     its gradient w.r.t. one fake tap, with the content loss's folded in at relu5_1, added to the VGG L1's;
 //   mg_pixel_l1_fwd/bwd   the background (masked) and rgb L1 losses on the images (loss.py:388-400, pix2pix_model.py:328-333).
@@ -196,6 +197,18 @@ __device__ __forceinline__ float lab_f(float t) { return t > kLabT ? powf(t, 1.f
 __device__ __forceinline__ float lab_df(float t, float ft) { return t > kLabT ? ft / (3.f * t) : 7.787f; }
 __device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
 
+// Chain rule from (a, b) to the image: o[c * plane] = scale * d(ca a + cb b) / d img_c at a pixel with xyz t and f(t) = ft.
+__device__ __forceinline__ void lab_ab_backprop(const float t[3], const float ft[3], float ca, float cb, float scale, float* o,
+                                                size_t plane) {
+    // d/d f(X), f(Y), f(Z), then through f' and the row-normalised M; d rgb / d img = 1/2
+    const float dfk[3] = {500.f * ca, -500.f * ca + 200.f * cb, -200.f * cb};
+    float dt[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) dt[k] = dfk[k] * lab_df(t[k], ft[k]) / ((kLabM[k][0] + kLabM[k][1]) + kLabM[k][2]);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c * plane] = scale * 0.5f * (dt[0] * kLabM[0][c] + dt[1] * kLabM[1][c] + dt[2] * kLabM[2][c]);
+}
+
 // sums[0] += sum over pixels of |a_fake - a_real| + |b_fake - b_real|  (fp64, caller zeroes)
 __global__ void __launch_bounds__(256) lab_loss_fwd_kernel(const float* __restrict__ fake, const float* __restrict__ real,
                                                            double* __restrict__ sums, int N, long long HW) {
@@ -238,14 +251,96 @@ __global__ void __launch_bounds__(256) lab_loss_bwd_kernel(const float* __restri
         for (int k = 0; k < 3; ++k) { ff[k] = lab_f(tf[k]); fr[k] = lab_f(tr[k]); }
         const float sa = sgn(500.f * (ff[0] - ff[1]) - 500.f * (fr[0] - fr[1]));
         const float sb = sgn(200.f * (ff[1] - ff[2]) - 200.f * (fr[1] - fr[2]));
-        // d/d f(X), f(Y), f(Z), then through f' and the row-normalised M; d rgb / d img = 1/2
-        const float dfk[3] = {500.f * sa, -500.f * sa + 200.f * sb, -200.f * sb};
-        float dt[3];
+        lab_ab_backprop(tf, ff, sa, sb, g, dfake + (size_t)n * 3 * HW + p, (size_t)HW);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ hair-average Lab loss
+// HairAvgLabLoss (loss.py:571-577, 601-621): avg = sum(Lab * m) / sum(m) per image (a mask sum of 0 counts as 1), L1 over the
+// a, b averages of fake and real.  Grid (blocks per image, N); every block reduces its share of one image in a fixed order and
+// writes its 8 partial sums, then hair_avg_lab_sum_kernel adds the partials of each image in a fixed order: no atomics, so two
+// runs give the same bits.  Per image: [fake: m L, m a, m b, m | real: the same] (each product rounded to fp32 first, as
+// torch's `input * mask`).
+constexpr int kHairVals = 8;
+
+__global__ void __launch_bounds__(256) hair_avg_lab_part_kernel(const float* __restrict__ fake, const float* __restrict__ real,
+                                                                const float* __restrict__ mfake, const float* __restrict__ mreal,
+                                                                double* __restrict__ part, long long HW) {
+    const int n = blockIdx.y;
+    double s[kHairVals];
 #pragma unroll
-        for (int k = 0; k < 3; ++k) dt[k] = dfk[k] * lab_df(tf[k], ff[k]) / ((kLabM[k][0] + kLabM[k][1]) + kLabM[k][2]);
-        float* o = dfake + (size_t)n * 3 * HW + p;
+    for (int k = 0; k < kHairVals; ++k) s[k] = 0.0;
+    for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
 #pragma unroll
-        for (int c = 0; c < 3; ++c) o[c * HW] = g * 0.5f * (dt[0] * kLabM[0][c] + dt[1] * kLabM[1][c] + dt[2] * kLabM[2][c]);
+        for (int i = 0; i < 2; ++i) {
+            const float m = __ldg((i ? mreal : mfake) + (size_t)n * HW + p);
+            if (m == 0.f) continue;
+            float t[3], f[3];
+            lab_xyz((i ? real : fake) + (size_t)n * 3 * HW, (size_t)HW, (size_t)p, t);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) f[k] = lab_f(t[k]);
+            // loss.py:563-569: L = 116 f(Y) - 16 above the threshold, 903.3 Y below
+            const float L = t[1] > kLabT ? 116.f * f[1] - 16.f : 903.3f * t[1];
+            s[4 * i + 0] += (double)__fmul_rn(L, m);
+            s[4 * i + 1] += (double)__fmul_rn(500.f * (f[0] - f[1]), m);
+            s[4 * i + 2] += (double)__fmul_rn(200.f * (f[1] - f[2]), m);
+            s[4 * i + 3] += (double)m;
+        }
+    }
+    __shared__ double red[8][kHairVals];
+#pragma unroll
+    for (int k = 0; k < kHairVals; ++k) {
+        for (int off = 16; off > 0; off >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], off);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][k] = s[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < kHairVals) {
+        double t = 0.0;
+        for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
+        part[((size_t)n * gridDim.x + blockIdx.x) * kHairVals + threadIdx.x] = t;
+    }
+}
+
+// One block per image, one warp per value: sums[n][k] = sum over the image's nb partials, in a fixed order.
+__global__ void __launch_bounds__(256) hair_avg_lab_sum_kernel(const double* __restrict__ part, double* __restrict__ sums, int nb) {
+    const int n = blockIdx.x, k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const double* p = part + (size_t)n * nb * kHairVals + k;
+    double s = 0.0;
+    for (int b = lane; b < nb; b += 32) s += p[(size_t)b * kHairVals];
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    if (lane == 0) sums[(size_t)n * kHairVals + k] = s;
+}
+
+// dfake = mask_fake * (T[n][0] da/dimg + T[n][1] db/dimg), T[n][j] = g / (2N) sgn(avg_f - avg_r) / cnt_f, formed per block
+// from the image's sums (loss.py:575 replaces a zero mask sum by 1).
+__global__ void __launch_bounds__(256) hair_avg_lab_bwd_kernel(const float* __restrict__ fake, const float* __restrict__ mfake,
+                                                               const double* __restrict__ sums, const float* __restrict__ gscale,
+                                                               float* __restrict__ dfake, long long HW) {
+    const int n = blockIdx.y;
+    __shared__ float tab[2];
+    if (threadIdx.x < 2) {
+        const double* s = sums + (size_t)n * kHairVals;
+        const double cf = s[3] == 0.0 ? 1.0 : s[3], cr = s[7] == 0.0 ? 1.0 : s[7];
+        const double d = s[1 + threadIdx.x] / cf - s[5 + threadIdx.x] / cr;
+        const double sg = d > 0.0 ? 1.0 : (d < 0.0 ? -1.0 : 0.0);
+        tab[threadIdx.x] = (float)((double)__ldg(gscale) / (2.0 * gridDim.y) * sg / cf);
+    }
+    __syncthreads();
+    const float ta = tab[0], tb = tab[1];
+    const float* img = fake + (size_t)n * 3 * HW;
+    float* out = dfake + (size_t)n * 3 * HW;
+    for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
+        const float m = __ldg(mfake + (size_t)n * HW + p);
+        if (m == 0.f) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) out[c * HW + p] = 0.f;
+            continue;
+        }
+        float t[3], f[3];
+        lab_xyz(img, (size_t)HW, (size_t)p, t);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) f[k] = lab_f(t[k]);
+        lab_ab_backprop(t, f, ta, tb, m, out + p, (size_t)HW);
     }
 }
 
@@ -464,6 +559,42 @@ extern "C" int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, c
     lab_loss_bwd_kernel<<<grid_for((long long)N * H * W), 256, 0, ST(stream)>>>(fake_nchw, real_nchw, gscale, dfake_nchw, N,
                                                                                (long long)H * W);
     return check_launch("mg_lab_loss_bwd");
+}
+
+// blocks per image of the hair-average kernels: enough to fill the GPU, no more than the image has 256-pixel chunks
+static int hair_blocks(int N, long long HW) {
+    long long b = (HW + 255) / 256;
+    const long long cap = ((long long)num_sms() * 8 + N - 1) / N;
+    if (b > cap) b = cap;
+    return (int)(b < 1 ? 1 : b);
+}
+
+extern "C" int mg_hair_avg_lab_fwd(const float* fake_nchw, const float* real_nchw, const float* mask_fake, const float* mask_real,
+                                   double* sums, int N, int H, int W, void* stream) {
+    if (!fake_nchw || !real_nchw || !mask_fake || !mask_real || !sums) return set_error(-1, "mg_hair_avg_lab_fwd: null pointer");
+    if (N < 1 || N > 65535 || H < 1 || W < 1) return set_error(-2, "mg_hair_avg_lab_fwd: bad size");
+    const long long HW = (long long)H * W;
+    const int nb = hair_blocks(N, HW);
+    double* part = nullptr;
+    int rc = acc64_alloc(&part, (size_t)N * nb * kHairVals, ST(stream));
+    if (rc) return rc;
+    hair_avg_lab_part_kernel<<<dim3(nb, N), 256, 0, ST(stream)>>>(fake_nchw, real_nchw, mask_fake, mask_real, part, HW);
+    rc = check_launch("mg_hair_avg_lab_fwd");
+    if (!rc) {
+        hair_avg_lab_sum_kernel<<<N, 32 * kHairVals, 0, ST(stream)>>>(part, sums, nb);
+        rc = check_launch("mg_hair_avg_lab_fwd");
+    }
+    const int rc2 = acc64_free(part, ST(stream));
+    return rc ? rc : rc2;
+}
+
+extern "C" int mg_hair_avg_lab_bwd(const float* fake_nchw, const float* mask_fake, const double* sums, const float* gscale,
+                                   float* dfake_nchw, int N, int H, int W, void* stream) {
+    if (!fake_nchw || !mask_fake || !sums || !gscale || !dfake_nchw) return set_error(-1, "mg_hair_avg_lab_bwd: null pointer");
+    if (N < 1 || N > 65535 || H < 1 || W < 1) return set_error(-2, "mg_hair_avg_lab_bwd: bad size");
+    const long long HW = (long long)H * W;
+    hair_avg_lab_bwd_kernel<<<dim3(hair_blocks(N, HW), N), 256, 0, ST(stream)>>>(fake_nchw, mask_fake, sums, gscale, dfake_nchw, HW);
+    return check_launch("mg_hair_avg_lab_bwd");
 }
 
 extern "C" int mg_style_loss_fwd(const void* taps_host, int n_taps, double* loss, void* stream) {

@@ -60,10 +60,11 @@ def install(reference_root=None, compat=True):
         setattr(sbn, name, getattr(mine.sync_batchnorm, name))
     pkg.SPADEBGenerator, pkg.MultiscaleDiscriminator, pkg.NLayerDiscriminator = G, MSD, NLD
     # the perceptual, style / content, background and Lab colour losses (pix2pix_model.py:41-53 look them up as networks.VGGLoss,
-    # networks.StyleContentLoss, networks.RGBBackgroundL1Loss, networks.LabColorLoss).  The rgb term is a bare nn.L1Loss
-    # (pix2pix_model.py:51) and stays torch's: torch.nn is not patched.
+    # networks.StyleContentLoss, networks.RGBBackgroundL1Loss, networks.LabColorLoss) and the hair-average Lab loss of the
+    # unpaired stage (pix2pix_model.py:55-56, networks.HairAvgLabLoss).  The rgb term is a bare nn.L1Loss (pix2pix_model.py:51)
+    # and stays torch's: torch.nn is not patched.
     los = importlib.import_module("models.networks.loss")
-    for name in ("VGGLoss", "StyleContentLoss", "RGBBackgroundL1Loss", "LabColorLoss"):
+    for name in ("VGGLoss", "StyleContentLoss", "RGBBackgroundL1Loss", "LabColorLoss", "HairAvgLabLoss"):
         setattr(los, name, getattr(mine.loss, name))
         setattr(pkg, name, getattr(mine.loss, name))
     if getattr(gen, "InpaintGenerator", None) is not None:
@@ -81,11 +82,13 @@ def _patch_runtime():
 
       * `util.save_network` (util/util.py:195-200) -> michigan_b200.checkpoint.save_network: rank 0 only, atomic rename,
         barrier, no round trip of the whole network through the CPU;
-      * `Pix2PixModel.compute_generator_loss` (pix2pix_model.py:257-365): the discriminator's parameters do not require
-        grad while the GENERATOR's loss is back-propagated - the reference computes those gradients and throws them
-        away (optimizer_D.zero_grad() runs before they could be used, pix2pix_trainer.py:62-69), here they are not
-        computed (and not all-reduced) at all.  Gradient averaging itself needs no hook: it happens inside backward()
-        (networks/sync_batchnorm.GradReducer), so the unchanged Pix2PixTrainer is data-parallel as is."""
+      * `Pix2PixModel.compute_generator_loss` (pix2pix_model.py:257-365): the discriminators' parameters (netD, and netD2
+        of --unpairTrain, which judges the generator in the unpaired stage, pix2pix_model.py:568-572) do not require grad
+        while the GENERATOR's loss is back-propagated - the reference computes those gradients and throws them away
+        (optimizer_D.zero_grad() / optimizer_D2.zero_grad() run before they could be used, pix2pix_trainer.py:61-77), here
+        they are not computed (and not all-reduced) at all.  Gradient averaging itself needs no hook: it happens inside
+        backward() (networks/sync_batchnorm.GradReducer, one per network), so the unchanged Pix2PixTrainer is data-parallel
+        as is."""
     from . import checkpoint
     util_mod = importlib.import_module("util.util")
     util_mod.save_network = checkpoint.save_network
@@ -95,8 +98,8 @@ def _patch_runtime():
         orig = cls.compute_generator_loss
 
         def compute_generator_loss(self, *a, **k):
-            netD = getattr(self, "netD", None)
-            flags = [(p, p.requires_grad) for p in netD.parameters()] if netD is not None else []
+            nets = [n for n in (getattr(self, "netD", None), getattr(self, "netD2", None)) if n is not None]
+            flags = [(p, p.requires_grad) for n in nets for p in n.parameters()]
             for p, _ in flags:
                 p.requires_grad_(False)
             try:

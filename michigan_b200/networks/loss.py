@@ -438,6 +438,43 @@ class LabColorLoss(nn.Module):
         return _LabLossFn.apply(fake, real.float())
 
 
+class _HairAvgLabFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, fake, real, mask_fake, mask_real):
+        f, mf = fake.detach().contiguous(), mask_fake.detach().contiguous()
+        sums = ops.hair_avg_lab_fwd(f, real.detach().contiguous(), mf, mask_real.detach().contiguous())
+        ctx.save_for_backward(f, mf, sums)
+        cnt = sums[:, :, 3:]
+        avg = sums[:, :, 1:3] / torch.where(cnt == 0, torch.ones_like(cnt), cnt)       # loss.py:575
+        return (avg[:, 0] - avg[:, 1]).abs().mean().float()
+
+    @staticmethod
+    def backward(ctx, g):
+        f, mf, sums = ctx.saved_tensors
+        return ops.hair_avg_lab_bwd(f, mf, sums, g.float().reshape(1).contiguous()), None, None, None
+
+
+class HairAvgLabLoss(nn.Module):
+    """loss.py:534-621 with balance_Lab=False: L1 between the hair-averaged a, b of fake (tag hair mask_fake) and of
+    real.detach() (reference hair mask_real), avg = sum(Lab * m) / sum(m), a mask sum of 0 counted as 1.  One fused kernel
+    pair each way (csrc/mg_vgg.cu: mg_hair_avg_lab_fwd, mg_hair_avg_lab_bwd)."""
+
+    def __init__(self, opt):
+        super().__init__()
+        if getattr(opt, "balance_Lab", False):
+            raise NotImplementedError("michigan_b200: --balance_Lab is not implemented (it needs data/ab_count.npy and grid_sample)")
+        self.opt = opt
+
+    def forward(self, fake, real, mask_fake, mask_real):
+        if fake.shape != real.shape or fake.shape[1] != 3:
+            raise ValueError("HairAvgLabLoss: expected two [N,3,H,W] images, got %s and %s" % (tuple(fake.shape), tuple(real.shape)))
+        n, _, h, w = fake.shape
+        for name, m in (("mask_fake", mask_fake), ("mask_real", mask_real)):
+            if tuple(m.shape) != (n, 1, h, w):
+                raise ValueError("HairAvgLabLoss: %s must be [N,1,H,W] = %s, got %s" % (name, (n, 1, h, w), tuple(m.shape)))
+        return _HairAvgLabFn.apply(fake, real.float(), mask_fake.float(), mask_real.float())
+
+
 class L1OLoss(nn.Module):
     """loss.py:274-385 with orient_filter='gabor': (orient_loss, confidence_loss) = forward(fake_image, orientation_label,
     input_semantics).  orientation_label: the 1-channel angle map (0..255) or, with --use_ig, the 2-channel (sin 2t, cos 2t) map."""

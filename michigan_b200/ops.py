@@ -696,6 +696,29 @@ def lab_loss_bwd(fake, real, gscale):
     return dfake
 
 
+def hair_avg_lab_fwd(fake, real, mask_fake, mask_real):
+    """-> [N,2,4] float64 device tensor: per image (sum m L, sum m a, sum m b, sum m) of fake with mask_fake, then of real with
+    mask_real (NCHW images in [-1, 1], masks [N,1,H,W])."""
+    _chk(fake, "fake"); _chk(real, "real"); _chk(mask_fake, "mask_fake"); _chk(mask_real, "mask_real")
+    N, _, H, W = fake.shape
+    assert fake.shape == real.shape and fake.shape[1] == 3, (fake.shape, real.shape)
+    assert tuple(mask_fake.shape) == tuple(mask_real.shape) == (N, 1, H, W), (mask_fake.shape, mask_real.shape)
+    sums = torch.empty((N, 2, 4), device=fake.device, dtype=torch.float64)
+    check(_lib.load().mg_hair_avg_lab_fwd(_p(fake), _p(real), _p(mask_fake), _p(mask_real), _p(sums), N, H, W, _stream()),
+          "mg_hair_avg_lab_fwd")
+    return sums
+
+
+def hair_avg_lab_bwd(fake, mask_fake, sums, g):
+    """d fake [N,3,H,W] of g[0] * the hair-average Lab loss given hair_avg_lab_fwd's sums; g: [1] fp32 device tensor."""
+    _chk(fake, "fake"); _chk(mask_fake, "mask_fake"); _chk(sums, "sums", torch.float64); _chk(g, "g")
+    N, _, H, W = fake.shape
+    dfake = torch.empty_like(fake)
+    check(_lib.load().mg_hair_avg_lab_bwd(_p(fake), _p(mask_fake), _p(sums), _p(g), _p(dfake), N, H, W, _stream()),
+          "mg_hair_avg_lab_bwd")
+    return dfake
+
+
 class StyleTap(C.Structure):
     """One record of mg_style_loss_fwd's host table (include/michigan_b200.h)."""
     _fields_ = [("sums_f", C.c_void_p), ("sums_t", C.c_void_p), ("coef", C.c_void_p), ("M", C.c_longlong), ("N", C.c_int32),
