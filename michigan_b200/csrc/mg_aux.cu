@@ -598,10 +598,11 @@ __global__ void bn_finalize_kernel(const double* __restrict__ sums, int C, doubl
     nshift[c] = (float)(-mean * rstd);
     if (mean_out) mean_out[c] = (float)mean;
     if (var_out) var_out[c] = (float)var;
-    if (rmean) rmean[c] = (1.f - momentum) * rmean[c] + momentum * (float)mean;
+    // batchnorm.py:139-143 as eager fp32 ops: (1 - m) * running + m * stat, both products rounded before the add
+    if (rmean) rmean[c] = __fadd_rn(__fmul_rn(1.f - momentum, rmean[c]), __fmul_rn(momentum, (float)mean));
     if (rvar) {
         const double unb = count_u > 1.0 ? var * count_u / (count_u - 1.0) : var;
-        rvar[c] = (1.f - momentum) * rvar[c] + momentum * (float)unb;
+        rvar[c] = __fadd_rn(__fmul_rn(1.f - momentum, rvar[c]), __fmul_rn(momentum, (float)unb));
     }
 }
 
@@ -713,7 +714,7 @@ __global__ void prep_bginput_kernel(const float* __restrict__ img, const float* 
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
             const size_t o = ((size_t)n * 3 + c) * HW + p;
-            v[c] = img[o] * bm + noise[o] * (1.f - bm);
+            v[c] = __fadd_rn(__fmul_rn(img[o], bm), __fmul_rn(noise[o], 1.f - bm));   // encoder.py:321's eager order
         }
         reinterpret_cast<float4*>(out4)[idx] = make_float4(v[0], v[1], v[2], 0.f);
     }
@@ -733,7 +734,8 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ in, float* __restr
 }
 
 // PartialConv2d mask bookkeeping (partialconv2d.py:57-66), single-channel mask [N,H,W]:
-// um = sum of mask over the k x k window (zero padded); ratio = k*k/(um+1e-8)*clamp(um,0,1); update = clamp(um,0,1)
+// um = sum of mask over the k x k window (zero padded); ratio = k*k/(um+1e-8)*clamp(um,0,1); update = clamp(um,0,1).
+// The reference's `slide_winsize / t` is a Python float over a tensor, which torch evaluates as t.reciprocal() * slide_winsize.
 __global__ void partial_mask_kernel(const float* __restrict__ mask, float* __restrict__ ratio, float* __restrict__ update,
                                     int N, int H, int W, int OH, int OW, int k, int s, int p) {
     const long long total = (long long)N * OH * OW;
@@ -752,7 +754,7 @@ __global__ void partial_mask_kernel(const float* __restrict__ mask, float* __res
                 um += mask[((size_t)n * H + ih) * W + iw];
             }
         }
-        const float r = (float)(k * k) / (um + 1e-8f);
+        const float r = __fmul_rn(__frcp_rn(um + 1e-8f), (float)(k * k));
         const float u = fminf(fmaxf(um, 0.f), 1.f);
         ratio[idx] = r * u;
         update[idx] = u;

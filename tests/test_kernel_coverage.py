@@ -1,0 +1,231 @@
+"""Every C entry point of the library is exercised by a GPU test, directly or through a Python wrapper.
+
+The entry points are the `int mg_*(` / `long long mg_*(` declarations of include/michigan_b200.h.  A tests/test_gpu_*.py module
+exercises one when its code (not its comments or docstrings) names the entry point itself, an ops.* wrapper that calls it
+(directly or through other ops.* functions), or a top-level class / function of the package that reaches it (e.g.
+SpectralNormBatch, LabColorLoss; not a whole network, see END_TO_END).  Package names count only as the module's imports
+bind them.  Entry points no such module reaches are listed in NOT_IN_GPU_TESTS with the reason.
+"""
+import ast
+import os
+import re
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "michigan_b200.h")
+PKG = os.path.join(ROOT, "michigan_b200")
+TESTS = os.path.join(ROOT, "tests")
+
+ENTRY_RE = re.compile(r"^\s*(?:int|long\s+long)\s+(mg_\w+)\s*\(", re.M)
+
+NOT_IN_GPU_TESTS = {
+    "mg_peer_allreduce_f64": "needs two GPUs: tests/nccl_worker.py runs it on 2 GPUs (launched by test_gpu_multi.py)",
+    "mg_peer_buffer_bytes": "size query of the 2-GPU all-reduce, called by tests/nccl_worker.py on 2 GPUs",
+    "mg_peer_max_elems": "size query of the 2-GPU all-reduce, called by tests/nccl_worker.py on 2 GPUs",
+    "mg_debug_igemm_prof": "probe counters, compiled only into the -DMG_PROBES build that tools/ load",
+    "mg_debug_seg_prof": "probe counters, compiled only into the -DMG_PROBES build that tools/ load",
+    "mg_version": "ABI query, checked by tests/test_abi.py",
+    "mg_launch_count": "ABI query, checked by tests/test_abi.py",
+    "mg_set_tuning": "ABI knob setter, checked by tests/test_abi.py",
+    "mg_get_tuning": "ABI knob getter, checked by tests/test_abi.py",
+    "mg_style_tap_bytes": "descriptor size query, checked against the ctypes layout by tests/test_abi.py",
+}
+
+
+# Whole networks and the training model run dozens of kernels end to end, under bounds loose enough to pass a kernel that is
+# wrong on one border or channel range: reaching an entry point only through one of them does not count.
+END_TO_END = {"BaseNetwork", "Pix2PixModel"}
+
+
+def entry_points():
+    with open(HEADER) as f:
+        return set(ENTRY_RE.findall(f.read()))
+
+
+def _code_names(tree):
+    """Identifiers a module's code uses: names and attribute names (strings, comments and docstrings do not count)."""
+    out = set()
+    for node in ast.walk(tree):
+        if isinstance(node, ast.Name):
+            out.add(node.id)
+        elif isinstance(node, ast.Attribute):
+            out.add(node.attr)
+        elif isinstance(node, ast.alias):
+            out.add(node.name.split(".")[-1])
+    return out
+
+
+def _parse(path):
+    with open(path) as f:
+        src = f.read()
+    return src, ast.parse(src)
+
+
+def ops_wrappers():
+    """ops.<function> -> entry points it calls, following calls to other ops functions."""
+    src, tree = _parse(os.path.join(PKG, "ops.py"))
+    funcs = {n.name: n for n in tree.body if isinstance(n, ast.FunctionDef)}
+    direct = {name: {a for a in _code_names(fn) if a.startswith("mg_")} for name, fn in funcs.items()}
+    calls = {name: {n.func.id for n in ast.walk(fn) if isinstance(n, ast.Call) and isinstance(n.func, ast.Name)
+                    and n.func.id in funcs} for name, fn in funcs.items()}
+    out = {}
+    for name in funcs:
+        seen, todo, eps = set(), [name], set()
+        while todo:
+            f = todo.pop()
+            if f in seen:
+                continue
+            seen.add(f)
+            eps |= direct[f]
+            todo.extend(calls[f])
+        out[name] = eps
+    return out
+
+
+def package_callers():
+    """Top-level classes and functions of the other package modules -> entry points their code reaches: the ones it names,
+    those of the ops.* wrappers it calls, and those of the other top-level classes / functions it uses."""
+    wrappers = ops_wrappers()
+    uses = {}
+    for dirpath, _, files in os.walk(PKG):
+        for fn in files:
+            if not fn.endswith(".py") or fn in ("ops.py", "_lib.py"):
+                continue
+            _, tree = _parse(os.path.join(dirpath, fn))
+            for node in tree.body:
+                if isinstance(node, ast.ClassDef) and (node.name in END_TO_END or
+                                                       any(getattr(bs, "id", None) in END_TO_END for bs in node.bases)):
+                    continue
+                if isinstance(node, (ast.ClassDef, ast.FunctionDef)):
+                    uses.setdefault(node.name, set()).update(_code_names(node))
+    out = {}
+    for name in uses:
+        seen, todo, eps = set(), [name], set()
+        while todo:
+            n = todo.pop()
+            if n in seen:
+                continue
+            seen.add(n)
+            for m in uses[n]:
+                if m.startswith("mg_"):
+                    eps.add(m)
+                elif m in uses:
+                    todo.append(m)
+                else:
+                    eps |= wrappers.get(m, set())
+        out[name] = eps
+    return out
+
+
+def _is_package_module(dotted):
+    rel = os.path.join(ROOT, *dotted.split("."))
+    return os.path.isfile(rel + ".py") or os.path.isfile(os.path.join(rel, "__init__.py"))
+
+
+def _test_module_reach(tree, wrappers, callers):
+    """Entry points a test module's code reaches, resolving names through its imports only: `mg_*` attributes (calls into
+    the loaded library), package modules bound by an import (also through a local getter such as `def _ops(): from
+    michigan_b200 import ops; return ops` and `ops = _ops()`) and their attributes, and classes / functions imported from
+    the package.  A local variable that happens to share a package name is not a package reference."""
+    modules, symbols = {}, {}
+    for node in ast.walk(tree):
+        if isinstance(node, ast.ImportFrom) and node.module and node.module.split(".")[0] == "michigan_b200":
+            for a in node.names:
+                full = node.module + "." + a.name
+                if _is_package_module(full):
+                    modules[a.asname or a.name] = full
+                else:
+                    symbols[a.asname or a.name] = (node.module, a.name)
+        elif isinstance(node, ast.Import):
+            for a in node.names:
+                if a.name.split(".")[0] == "michigan_b200" and a.asname:
+                    modules[a.asname] = a.name
+    getters = {}
+    for node in ast.walk(tree):
+        if isinstance(node, ast.FunctionDef):
+            for r in ast.walk(node):
+                if isinstance(r, ast.Return) and isinstance(r.value, ast.Name) and r.value.id in modules:
+                    getters[node.name] = modules[r.value.id]
+
+    def module_of(expr):
+        if isinstance(expr, ast.Name):
+            return modules.get(expr.id)
+        if isinstance(expr, ast.Call) and isinstance(expr.func, ast.Name):
+            return getters.get(expr.func.id)
+        return None
+
+    for node in ast.walk(tree):
+        if isinstance(node, ast.Assign):
+            pairs = [(node.targets[0], node.value)]
+            if isinstance(node.targets[0], ast.Tuple) and isinstance(node.value, ast.Tuple):
+                pairs = list(zip(node.targets[0].elts, node.value.elts))
+            for t, v in pairs:
+                m = module_of(v)
+                if m and isinstance(t, ast.Name):
+                    modules[t.id] = m
+
+    def resolve(module, name):
+        return wrappers.get(name, set()) if module == "michigan_b200.ops" else callers.get(name, set())
+
+    eps = set()
+    for node in ast.walk(tree):
+        if isinstance(node, ast.Attribute):
+            if node.attr.startswith("mg_"):
+                eps.add(node.attr)
+            m = module_of(node.value)
+            if m:
+                eps |= resolve(m, node.attr)
+        elif isinstance(node, ast.Name) and node.id in symbols:
+            eps |= resolve(*symbols[node.id])
+    return eps
+
+
+def exercised_by_gpu_tests():
+    """entry point -> the tests/test_gpu_*.py modules whose code reaches it."""
+    wrappers, callers = ops_wrappers(), package_callers()
+    reach = {}
+    for fn in sorted(os.listdir(TESTS)):
+        if not (fn.startswith("test_gpu_") and fn.endswith(".py")):
+            continue
+        _, tree = _parse(os.path.join(TESTS, fn))
+        for e in _test_module_reach(tree, wrappers, callers):
+            reach.setdefault(e, set()).add(fn)
+    return reach
+
+
+def test_header_lists_the_entry_points():
+    eps = entry_points()
+    assert len(eps) > 50, sorted(eps)
+    assert {"mg_conv_igemm", "mg_bn_stats", "mg_spectral_norm_batched", "mg_peer_allreduce_f64"} <= eps
+
+
+def test_ops_wrappers_call_declared_entry_points():
+    eps = entry_points()
+    w = ops_wrappers()
+    assert w["mlp_shared"] >= {"mg_conv_seg_tc", "mg_conv_thin"}
+    undeclared = {n: sorted(e - eps) for n, e in w.items() if e - eps}
+    assert not undeclared, undeclared
+
+
+def test_every_entry_point_is_exercised_by_a_gpu_test():
+    eps = entry_points()
+    reach = exercised_by_gpu_tests()
+    assert set(NOT_IN_GPU_TESTS) <= eps, sorted(set(NOT_IN_GPU_TESTS) - eps)
+    missing = sorted(e for e in eps if e not in reach and e not in NOT_IN_GPU_TESTS)
+    assert not missing, "entry points no tests/test_gpu_*.py module reaches (add a test or list them with a reason): %s" % missing
+    stale = sorted(e for e in NOT_IN_GPU_TESTS if e in reach)
+    assert not stale, "listed as untested but reached by a GPU test: %s" % stale
+
+
+def test_names_resolve_through_imports_only():
+    """A local variable named like a package class or ops function credits nothing; the imported name does."""
+    wrappers, callers = ops_wrappers(), package_callers()
+    assert callers["SPADE"], "SPADE reaches entry points through its convs"
+    local = ast.parse("SPADE = [1, 2]\nconv_thin = None\n\ndef test_x():\n    return SPADE, conv_thin\n")
+    assert _test_module_reach(local, wrappers, callers) == set()
+    imported = ast.parse("from michigan_b200.networks import SPADE\n\ndef test_x():\n    return SPADE\n")
+    assert _test_module_reach(imported, wrappers, callers) == callers["SPADE"]
+    getter = ast.parse("def _ops():\n    from michigan_b200 import ops\n    return ops\n\n"
+                       "def test_x():\n    ops = _ops()\n    ops.conv_thin(None)\n    _ops().maxpool_mask(None, 3)\n")
+    assert _test_module_reach(getter, wrappers, callers) == {"mg_conv_thin", "mg_maxpool_mask"}
+    direct = ast.parse("def test_x(lib):\n    lib.load().mg_edge_weight(0)\n")
+    assert _test_module_reach(direct, wrappers, callers) == {"mg_edge_weight"}
