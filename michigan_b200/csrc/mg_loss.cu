@@ -104,7 +104,9 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
     }
 }
 
-// ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * [sign*a - 1 < 0];  op 1: 1;  op 2: sgn(a - b);  op 3: 2 (a - b)
+// ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * ([sign*a - 1 < 0] + [sign*a - 1 == 0] / 2);  op 1: 1;
+// op 2: sgn(a - b);  op 3: 2 (a - b).  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0)) gives each side
+// half the gradient.
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
     const LossTerm t = terms[blockIdx.y];
     if (!t.ga) return;
@@ -112,7 +114,10 @@ __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
         const float a = __ldg(t.a + i);
         float d;
-        if (t.op == 0) d = (t.sign * a - 1.f < 0.f) ? t.sign * (t.b ? __ldg(t.b + i) : 1.f) : 0.f;
+        if (t.op == 0) {
+            const float m = t.sign * a - 1.f;
+            d = m < 0.f ? t.sign * (t.b ? __ldg(t.b + i) : 1.f) : (m == 0.f ? 0.5f * t.sign * (t.b ? __ldg(t.b + i) : 1.f) : 0.f);
+        }
         else if (t.op == 1) d = 1.f;
         else if (t.op == 2) { const float df = a - __ldg(t.b + i); d = df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f); }
         else d = 2.f * (a - __ldg(t.b + i));

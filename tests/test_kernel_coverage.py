@@ -31,6 +31,24 @@ NOT_IN_GPU_TESTS = {
 }
 
 
+# Tests that hold a kernel's every output element to a float64 reference (under a per-element bound) or to the bits of an
+# exact restatement.  Whole modules of such tests, then the named tests of modules that also hold end-to-end checks.
+ELEMENTWISE_MODULES = [
+    "test_gpu_backward_kernels.py",
+    "test_gpu_conv_forward_fp64.py",
+    "test_gpu_cuda_core_forward_fp64.py",
+    "test_gpu_loss_kernels_fp64.py",
+]
+ELEMENTWISE_TESTS = {
+    "test_gpu_style_content.py": ["test_style_kernels_vs_fp64_autograd", "test_pixel_l1_vs_fp64_autograd",
+                                  "test_content_op3_vs_fp64_autograd"],
+    "test_gpu_hair_avg_lab.py": ["test_hair_avg_lab_kernels_vs_fp64_autograd"],
+    "test_gpu_vgg_lab.py": ["test_maxpool2_forward_backward_vs_torch"],
+}
+# Entry points outside NOT_IN_GPU_TESTS that no element-wise test reaches, with the reason (none today).
+NOT_ELEMENTWISE = {}
+
+
 # Whole networks and the training model run dozens of kernels end to end, under bounds loose enough to pass a kernel that is
 # wrong on one border or channel range: reaching an entry point only through one of them does not count.
 END_TO_END = {"BaseNetwork", "Pix2PixModel"}
@@ -121,11 +139,25 @@ def _is_package_module(dotted):
     return os.path.isfile(rel + ".py") or os.path.isfile(os.path.join(rel, "__init__.py"))
 
 
-def _test_module_reach(tree, wrappers, callers):
+def _local_scope(tree, names):
+    """The module-level functions `names` and every module-level function or class they call by name, transitively."""
+    defs = {n.name: n for n in tree.body if isinstance(n, (ast.FunctionDef, ast.ClassDef))}
+    seen, todo = set(), [n for n in names if n in defs]
+    while todo:
+        n = todo.pop()
+        if n in seen:
+            continue
+        seen.add(n)
+        todo.extend(m for m in _code_names(defs[n]) if m in defs)
+    return [defs[n] for n in sorted(seen)]
+
+
+def _test_module_reach(tree, wrappers, callers, scope=None):
     """Entry points a test module's code reaches, resolving names through its imports only: `mg_*` attributes (calls into
     the loaded library), package modules bound by an import (also through a local getter such as `def _ops(): from
     michigan_b200 import ops; return ops` and `ops = _ops()`) and their attributes, and classes / functions imported from
-    the package.  A local variable that happens to share a package name is not a package reference."""
+    the package.  A local variable that happens to share a package name is not a package reference.  With `scope` (a list
+    of nodes of the module), only the code of those nodes counts; the imports are still resolved over the whole module."""
     modules, symbols = {}, {}
     for node in ast.walk(tree):
         if isinstance(node, ast.ImportFrom) and node.module and node.module.split(".")[0] == "michigan_b200":
@@ -167,7 +199,7 @@ def _test_module_reach(tree, wrappers, callers):
         return wrappers.get(name, set()) if module == "michigan_b200.ops" else callers.get(name, set())
 
     eps = set()
-    for node in ast.walk(tree):
+    for node in (n for s in (scope if scope is not None else [tree]) for n in ast.walk(s)):
         if isinstance(node, ast.Attribute):
             if node.attr.startswith("mg_"):
                 eps.add(node.attr)
@@ -214,6 +246,50 @@ def test_every_entry_point_is_exercised_by_a_gpu_test():
     assert not missing, "entry points no tests/test_gpu_*.py module reaches (add a test or list them with a reason): %s" % missing
     stale = sorted(e for e in NOT_IN_GPU_TESTS if e in reach)
     assert not stale, "listed as untested but reached by a GPU test: %s" % stale
+
+
+def exercised_by_elementwise_tests():
+    """entry point -> the element-wise tests (module, or module::function) whose code reaches it."""
+    wrappers, callers = ops_wrappers(), package_callers()
+    reach = {}
+    for fn in sorted(set(ELEMENTWISE_MODULES) | set(ELEMENTWISE_TESTS)):
+        _, tree = _parse(os.path.join(TESTS, fn))
+        if fn in ELEMENTWISE_MODULES:
+            scopes = {fn: None}
+        else:
+            defs = {n.name for n in tree.body if isinstance(n, ast.FunctionDef)}
+            missing = sorted(set(ELEMENTWISE_TESTS[fn]) - defs)
+            assert not missing, "%s has no test %s" % (fn, missing)
+            scopes = {fn + "::" + t: _local_scope(tree, [t]) for t in ELEMENTWISE_TESTS[fn]}
+        for name, scope in scopes.items():
+            for e in _test_module_reach(tree, wrappers, callers, scope):
+                reach.setdefault(e, set()).add(name)
+    return reach
+
+
+def test_every_entry_point_has_an_elementwise_test():
+    eps = entry_points()
+    reach = exercised_by_elementwise_tests()
+    for fn in set(ELEMENTWISE_MODULES) | set(ELEMENTWISE_TESTS):
+        assert os.path.isfile(os.path.join(TESTS, fn)), "element-wise test module %s is missing" % fn
+    assert set(NOT_ELEMENTWISE) <= eps, sorted(set(NOT_ELEMENTWISE) - eps)
+    missing = sorted(e for e in eps if e not in reach and e not in NOT_IN_GPU_TESTS and e not in NOT_ELEMENTWISE)
+    assert not missing, ("entry points no element-wise test reaches (add a float64 or bit-exact test, or list them in "
+                         "NOT_ELEMENTWISE with a reason): %s" % missing)
+    stale = sorted(e for e in NOT_ELEMENTWISE if e in reach)
+    assert not stale, "listed as without an element-wise test but reached by one: %s" % stale
+
+
+def test_elementwise_reach_is_per_function():
+    """Only the named functions of a mixed module count, with the module-level helpers they call; its other tests do not."""
+    wrappers, callers = ops_wrappers(), package_callers()
+    tree = ast.parse("from michigan_b200 import ops\n\n"
+                     "def _run(x):\n    return ops.conv_thin(x)\n\n"
+                     "def test_fp64():\n    _run(1)\n\n"
+                     "def test_end_to_end():\n    ops.maxpool_mask(None, 3)\n")
+    assert _test_module_reach(tree, wrappers, callers, _local_scope(tree, ["test_fp64"])) == {"mg_conv_thin"}
+    assert _test_module_reach(tree, wrappers, callers, _local_scope(tree, ["test_end_to_end"])) == {"mg_maxpool_mask"}
+    assert _test_module_reach(tree, wrappers, callers) == {"mg_conv_thin", "mg_maxpool_mask"}
 
 
 def test_names_resolve_through_imports_only():
