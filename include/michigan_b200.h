@@ -24,19 +24,17 @@
 extern "C" {
 #endif
 
-#define MG_ABI_VERSION 2
+#define MG_ABI_VERSION 3
 
 int mg_version(void);
 const char* mg_last_error(void);
 /* number of kernels this library has launched in the calling process (for bench.py's gpu_launches) */
 long long mg_launch_count(void);
-/* Schedule knobs ("MG_DUAL", "MG_MERGE", "MG_HALO", "MG_HALO_PW", "MG_EPI_IMPL", "MG_EPI_IMPL_SPADE", "MG_EPI_CW16",
- * "MG_EPI_CW_SPADE", "MG_STAGES", "MG_WGRAD_DUAL", "MG_THIN_GEMM", "MG_THIN_WGRAD_LEGACY", "MG_GROUP3", "MG_SEG_TMA", "MG_WGRAD_HALO", "MG_EPI_TMA", "MG_BN_FILL", "MG_EPI_EARLY", "MG_EPI_REG"): initialised once from the
+/* Schedule knobs ("MG_MERGE", "MG_HALO", "MG_HALO_PW", "MG_EPI_IMPL", "MG_EPI_IMPL_SPADE", "MG_EPI_CW16",
+ * "MG_EPI_CW_SPADE", "MG_STAGES", "MG_THIN_GEMM", "MG_GROUP3", "MG_SEG_TMA", "MG_BN_FILL", "MG_EPI_REG"): initialised once from the
  * environment variable of the same name, changed here by tests and A/B tools.  Unknown name: -2 / -1. */
 int mg_set_tuning(const char* name, int value);
 int mg_get_tuning(const char* name);
-/* debugging aid (probe build only, zeros otherwise): 16 clock64() totals CTA 0 of mg_conv_igemm recorded under env MG_DBG=16 */
-int mg_debug_igemm_prof(unsigned long long* host16);
 
 /* activation codes */
 #define MG_ACT_NONE 0
@@ -305,10 +303,6 @@ int mg_spectral_norm_bwd(const float* dwt, const float* w_orig, const float* u, 
                          double* dot_ws, float* dw, int O, long long K, int accumulate, void* stream);
 int mg_pack_weight_dgrad_gb(const float* wg, const float* wb, float* out, int C, int I, int BN, void* stream);
 int mg_unpack_wgrad_gb(const float* dw_packed, float* dwg, float* dwb, int C, int I, int BN, int accumulate, void* stream);
-
-/* [N,H,W,CinP] (CinP 4|8; H,W = size after the optional nearest down-sampling by seg_resize) -> TF32-rounded
- * [N,H+2p,W+2p,32] with zero channel padding and reflection padding p: operand of mg_conv_wgrad for the thin convs. */
-int mg_pad_channels32(const float* in, float* out, int N, int H, int W, int CinP, int seg_resize, int reflect_pad, void* stream);
 
 /* ---- self-attention of the InpaintGenerator (generator.py:467-485) --------------------------------------------------------
  * softmax(Q K^T) V runs as two mg_conv_igemm launches per image (1x1 convs whose weight operand is that image's K resp. V^T)

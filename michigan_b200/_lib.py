@@ -59,7 +59,6 @@ SIGNATURES = {
     "mg_launch_count": [],
     "mg_set_tuning": [C.c_char_p, _i],
     "mg_get_tuning": [C.c_char_p],
-    "mg_debug_igemm_prof": [C.c_void_p],
     "mg_conv_igemm": [C.POINTER(IgemmArgs), _p],
     "mg_pack_weight": [_p, _p, _i, _i, _i, _i, _p, _i, _p],
     "mg_pack_weight_gb": [_p, _p, _p, _i, _i, _i, _i, _i, _p],
@@ -90,7 +89,6 @@ SIGNATURES = {
     "mg_pack_weight_dgrad": [_p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     "mg_unpack_wgrad": [_p, _p, _i, _i, _i, _i, _i, _p],
     "mg_conv_wgrad": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p],
-    "mg_pad_channels32": [_p, _p, _i, _i, _i, _i, _i, _i, _p],
     "mg_spade_bwd": [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p],
     "mg_cvt16": [_p, _p, _ll, _i, _p],
     "mg_conv_wgrad16": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p],

@@ -35,12 +35,12 @@ int num_sms() {
 
 // ---------------------------------------------------------------------------------------------- tuning knobs
 struct KnobDef { const char* env; int dflt; };
-static const KnobDef kKnobs[TK_COUNT] = {
-    {"MG_DUAL", 2}, {"MG_MERGE", 1}, {"MG_HALO", 0}, {"MG_HALO_PW", 10}, {"MG_EPI_IMPL", 1}, {"MG_EPI_IMPL_SPADE", -1},
-    {"MG_EPI_CW16", 1}, {"MG_EPI_CW_SPADE", 16}, {"MG_STAGES", 0}, {"MG_WGRAD_DUAL", 1}, {"MG_THIN_GEMM", 1},
-    {"MG_THIN_WGRAD_LEGACY", 0}, {"MG_GROUP3", 1}, {"MG_SEG_TMA", 1}, {"MG_WGRAD_HALO", 1}, {"MG_EPI_TMA", 2}, {"MG_BN_FILL", 1}, {"MG_EPI_EARLY", 0},
-    {"MG_EPI_REG", 1},
+static const KnobDef kKnobs[] = {
+    {"MG_MERGE", 1}, {"MG_HALO", 0}, {"MG_HALO_PW", 10}, {"MG_EPI_IMPL", 1}, {"MG_EPI_IMPL_SPADE", -1},
+    {"MG_EPI_CW16", 1}, {"MG_EPI_CW_SPADE", 16}, {"MG_STAGES", 0}, {"MG_THIN_GEMM", 1},
+    {"MG_GROUP3", 1}, {"MG_SEG_TMA", 1}, {"MG_BN_FILL", 1}, {"MG_EPI_REG", 1},
 };
+static_assert(sizeof(kKnobs) / sizeof(kKnobs[0]) == TK_COUNT, "kKnobs needs one row per TuneKnob, in enum order");
 static std::atomic<int> g_knob[TK_COUNT];
 static std::once_flag g_knob_once;
 

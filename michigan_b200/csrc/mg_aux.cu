@@ -1307,42 +1307,3 @@ extern "C" int mg_pack_weight_gb16(const float* wg, const float* wb, void* out, 
     return check_launch("mg_pack_weight_gb16");
 }
 
-// ------------------------------------------------------------------------------------ channel padding to 32
-// out[n,i,j,0:32] = (c < CinP ? in[n, src_i, src_j, c] : 0) with optional nearest down-sampling by R (segmap) and
-// reflection padding by p (out is then [N,H+2p,W+2p,32]); values TF32-rounded: operand of the tensor-core weight-gradient
-// kernel for the thin (3/4/7-channel input) convolutions.
-namespace mg {
-__global__ void pad_channels32_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int H, int W, int CinP, int R,
-                                      int p) {
-    const int OH = H + 2 * p, OW = W + 2 * p;
-    const long long total = (long long)N * OH * OW * 8;   // float4 groups of 32 channels
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int g = idx & 7;
-        long long t = idx >> 3;
-        const int j = t % OW; t /= OW;
-        const int i = t % OH;
-        const int n = t / OH;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (g * 4 < CinP) {
-            int ih = i - p, iw = j - p;
-            if (ih < 0) ih = -ih;
-            if (ih >= H) ih = 2 * H - 2 - ih;
-            if (iw < 0) iw = -iw;
-            if (iw >= W) iw = 2 * W - 2 - iw;
-            v = __ldg(reinterpret_cast<const float4*>(in + (((size_t)n * H * R + (size_t)ih * R) * ((size_t)W * R) + (size_t)iw * R) * CinP) + g);
-            v.x = rtf32(v.x); v.y = rtf32(v.y); v.z = rtf32(v.z); v.w = rtf32(v.w);
-        }
-        reinterpret_cast<float4*>(out)[idx] = v;
-    }
-}
-}  // namespace mg
-extern "C" int mg_pad_channels32(const float* in, float* out, int N, int H, int W, int CinP, int seg_resize, int reflect_pad,
-                                 void* stream) {
-    if (!in || !out) return set_error(-1, "mg_pad_channels32: null pointer");
-    if (CinP != 4 && CinP != 8) return set_error(-2, "mg_pad_channels32: CinP must be 4 or 8");
-    const int R = seg_resize > 0 ? seg_resize : 1;
-    pad_channels32_kernel<<<ew_grid((long long)N * (H + 2 * reflect_pad) * (W + 2 * reflect_pad) * 8), 256, 0, ST(stream)>>>(
-        in, out, N, H, W, CinP, R, reflect_pad);
-    return check_launch("mg_pad_channels32");
-}

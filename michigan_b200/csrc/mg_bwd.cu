@@ -354,7 +354,7 @@ thin_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dz, dou
         for (int k = k0; k < k1; ++k) atomicAdd(dwt + (size_t)k * Cout + co, (double)acc[k - k0]);
 }
 
-// Register-tiled weight gradient of a thin conv (replaces the tensor-core route for Cin <= 8, which pads N to 32 channels).  Thread = (group of 4 output
+// Register-tiled weight gradient of a thin conv.  Thread = (group of 4 output
 // channels) x (KPT of the KH*KW*CinP weight columns): per pixel one float4 of dz and KPT input values from shared memory
 // feed 4*KPT FMAs; the per-CTA partial sums stay in registers across all its tiles and are added at the end into the fp64
 // accumulator of the launcher (acc64_*: the result does not depend on the order in which CTAs finish).
@@ -1009,8 +1009,7 @@ extern "C" int mg_thin_wgrad(const float* x, const float* dz, float* dwt, int N,
     // register-tiled kernel: Cout 64/128, columns per thread = ceil(K / (256 / (Cout/4)))
     const int CG = Cout == 64 || Cout == 128 ? 256 / (Cout / 4) : 0;
     const int kpt = CG ? (K + CG - 1) / CG : 0;
-    const bool legacy = tune(TK_THIN_WGRAD_LEGACY) != 0;
-    if (CG && kpt <= 13 && CinP % 4 == 0 && !legacy) {
+    if (CG && kpt <= 13 && CinP % 4 == 0) {
         const size_t smem = ((((size_t)PH * PW * CinP + 3) & ~(size_t)3) + 128 * (size_t)Cout) * 4;
         // load -> sync -> compute per tile: co-resident CTAs overlap one's loads with another's FMAs
         int per_sm = (int)((200 * 1024) / (smem + 1024));

@@ -57,7 +57,7 @@ struct IgemmParams {
     int acc_off, acc_ld;               // smem accumulator tile: byte offset, row pitch in floats (acc_cols + 4: conflict-free rows)
     // halo mode (3x3, stride 1, pad 1): one [PW x (TH+2)] input patch per K chunk serves all 9 taps
     int halo, PW, patch_bytes, patch_tx, a_slots, b_slots, b_slot_bytes, acc_cols, merged, n_items, bar_off;
-    int dbg;   // what-if probes (env MG_DBG; 1..8 give WRONG results): 1 no B loads after the first tile, 2 no A loads, 4 no epilogue work, 8 no epilogue global traffic (32 no 16-bit stores only, 64 no x loads only), 16 cycle profile
+    int dbg;   // what-if probes (env MG_DBG; 1..8 give WRONG results): 1 no B loads after the first tile, 2 no A loads, 4 no epilogue work, 8 no epilogue global traffic (32 no 16-bit stores only, 64 no x loads only)
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {

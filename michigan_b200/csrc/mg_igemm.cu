@@ -33,9 +33,6 @@
 
 namespace mg {
 
-// role-profile counters read by mg_debug_igemm_prof
-__device__ unsigned long long g_igemm_prof[16];
-
 // 16 consecutive channels -> 16-bit hi (and optional lo = cvt(y - hi)) copies, 32 B each.
 __device__ __forceinline__ void store16(const IgemmParams& p, const float (&y)[16], size_t elem_off) {
     uint32_t hi[8], lo[8];
@@ -643,15 +640,6 @@ int igemm_launch(const mg_igemm_args* a, cudaStream_t stream) {
 }
 
 }  // namespace mg
-
-// Debug: copy the 16 role-profile counters (synchronises).  The sm_90 kernel records none: all zero.
-extern "C" int mg_debug_igemm_prof(unsigned long long* host16) {
-    if (!host16) return mg::set_error(-1, "mg_debug_igemm_prof: null pointer");
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpyFromSymbol(host16, mg::g_igemm_prof, 16 * sizeof(unsigned long long));
-    if (e != cudaSuccess) return mg::set_error((int)e, "mg_debug_igemm_prof: %s", cudaGetErrorString(e));
-    return 0;
-}
 
 extern "C" int mg_conv_igemm(const mg_igemm_args* a, void* stream) {
     return mg::igemm_launch(a, reinterpret_cast<cudaStream_t>(stream));

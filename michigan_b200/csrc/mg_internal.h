@@ -17,8 +17,7 @@ int encode_tensor_map(CUtensorMap* map, void* gaddr, CUtensorMapDataType dtype, 
 // Tuning knobs (alternative schedules that all give the same results): read ONCE from the environment at first use,
 // overridable through mg_set_tuning() (tests, A/B tools).  Nothing on the launch path calls getenv.
 enum TuneKnob {
-    TK_DUAL = 0,         // MG_DUAL: accepted, no effect on sm_90a
-    TK_MERGE,            // MG_MERGE: split-precision convs with 2*BN <= 128 as two MMAs per K step (default 1)
+    TK_MERGE = 0,        // MG_MERGE: split-precision convs with 2*BN <= 128 as two MMAs per K step (default 1)
     TK_HALO,             // MG_HALO: halo schedule of 3x3/s1 convs (default 0)
     TK_HALO_PW,          // MG_HALO_PW: patch pitch 10 | 16
     TK_EPI_IMPL,         // MG_EPI_IMPL: 1 transposed epilogue (default), 0 row-per-lane reference epilogue
@@ -26,15 +25,10 @@ enum TuneKnob {
     TK_EPI_CW16,         // MG_EPI_CW16: 16-channel epilogue chunks (default 1)
     TK_CW_SPADE,         // MG_EPI_CW_SPADE: 16 | 32
     TK_STAGES,           // MG_STAGES: cap on the smem ring depth (0 = none)
-    TK_WGRAD_DUAL,       // MG_WGRAD_DUAL: accepted, no effect on sm_90a
     TK_THIN_GEMM,        // MG_THIN_GEMM (default 1)
-    TK_THIN_WGRAD_LEGACY,// MG_THIN_WGRAD_LEGACY (default 0)
     TK_GROUP3,           // MG_GROUP3: 3x3/s1 convs on the halo-patch + M-tile-group kernel (mg_conv3x3.cu): 0 off, 1 / 2 on
     TK_SEG_TMA,          // MG_SEG_TMA: 16-bit outputs of the seg conv through smem staging + TMA stores (default 1)
-    TK_WGRAD_HALO,       // MG_WGRAD_HALO: accepted, no effect on sm_90a
-    TK_EPI_TMA,          // MG_EPI_TMA: accepted, no effect on sm_90a
     TK_BN_FILL,          // MG_BN_FILL: generic convs whose tiles do not fill the SMs use a narrower BN (default 1)
-    TK_EPI_EARLY,        // MG_EPI_EARLY: accepted, no effect on sm_90a
     TK_EPI_REG,          // MG_EPI_REG: epilogue of the 3x3 group kernel on the accumulator registers (default 1), 0 through smem
     TK_COUNT
 };

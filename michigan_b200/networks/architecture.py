@@ -72,7 +72,7 @@ class SPADEResnetBlock(nn.Module):
         else:
             wgb = c.get((name + ".gb16", gfmt, gsplit), [sp.mlp_gamma.weight, sp.mlp_beta.weight],
                         lambda: ops.pack_weight_gb16(sp.mlp_gamma.weight.detach(), sp.mlp_beta.weight.detach(), gfmt, gsplit))
-        wsh = c.get((name + ".sh", ops.seg_tc_enabled()), [sp.mlp_shared[0].weight],
+        wsh = c.get(name + ".sh", [sp.mlp_shared[0].weight],
                     lambda: ops.pack_mlp_shared(sp.mlp_shared[0].weight.detach()))
         g1 = c.get(name + ".g1", [sp.mlp_gamma.bias], lambda: (sp.mlp_gamma.bias.detach() + 1.0).contiguous())
         return wsh, sp.mlp_shared[0].bias.detach(), wgb, g1, sp.mlp_beta.bias.detach()

@@ -80,7 +80,7 @@ def _conv_param_grads(G, conv, inv_of, dy, a_operand, kh, kw, stride, pad, with_
 
 
 # =============================================================================================== SPADE + conv
-def _spade_conv_bwd(G, blk, S, conv, inv_of, dy, k, pad, seg4, seg_cache=None):
+def _spade_conv_bwd(G, blk, S, conv, inv_of, dy, k, pad, seg4):
     """Backward of conv(act(SPADE(src))) given dy; returns (dxhat, sums) for the BN backward of `src`."""
     # bf16 gradient GEMMs: dY's bf16 copy and (for convs with a bias) its channel sums come out of one pass over dY
     dy16 = bias_sum = None
@@ -115,21 +115,9 @@ def _spade_conv_bwd(G, blk, S, conv, inv_of, dy, k, pad, seg4, seg_cache=None):
     G.add(sp.mlp_gamma.bias, bsum[:c].float())
     G.add(sp.mlp_beta.bias, bsum[c:].float())
     del dgb
-    if ops.thin_wgrad_tc_enabled():
-        da = ops.act_bwd(dactv, actv, _RELU)
-        del dactv, actv
-        seg32 = seg_cache.get(S.R) if seg_cache is not None else None
-        if seg32 is None:
-            seg32 = ops.pad_channels32(seg4, seg_resize=S.R, in_hw=S.hw)
-            if seg_cache is not None:
-                seg_cache.clear()          # one resolution at a time is alive (blocks run coarse -> fine in reverse)
-                seg_cache[S.R] = seg32
-        dwt = ops.thin_wgrad_tc(seg32, da, 3, 3, 1, 1, 4)
-        db = ops.chan_sum(da)
-    else:
-        # ReLU backward of mlp_shared and its bias gradient are fused into the weight-gradient kernel: d actv is read once
-        dwt, db = ops.thin_wgrad(seg4, dactv, 3, 3, 1, 1, seg_resize=S.R, in_hw=S.hw, relu_src=actv, want_bias=True)
-        del dactv, actv
+    # ReLU backward of mlp_shared and its bias gradient are fused into the weight-gradient kernel: d actv is read once
+    dwt, db = ops.thin_wgrad(seg4, dactv, 3, 3, 1, 1, seg_resize=S.R, in_hw=S.hw, relu_src=actv, want_bias=True)
+    del dactv, actv
     G.add(sp.mlp_shared[0].weight, _thin_wt_to_oihw(dwt, 3, 3, 4))
     G.add(sp.mlp_shared[0].bias, db)
     return dxhat, sums, allreduce_sums(sums, dxhat.numel() // c)
@@ -138,22 +126,21 @@ def _spade_conv_bwd(G, blk, S, conv, inv_of, dy, k, pad, seg4, seg_cache=None):
 # =============================================================================================== SPADEResnetBlock
 def block_bwd(G, blk, S, dout, seg4, inv_of):
     """-> (dx wrt the block input (pre-upsample), dbf wrt the blended background feature or None)."""
-    seg_cache = {}
     dbf = None
     if S.blend is not None:
         _, hair, back, ms = S.blend
         dy, dbf = ops.blend_bwd(dout, hair, back, ms)
     else:
         dy = dout
-    dxhat1, sums1, cnt1 = _spade_conv_bwd(G, blk, S.sp1, blk.conv_1, inv_of, dy, 3, 1, seg4, seg_cache)
+    dxhat1, sums1, cnt1 = _spade_conv_bwd(G, blk, S.sp1, blk.conv_1, inv_of, dy, 3, 1, seg4)
     ddx = ops.bn_bwd_apply(dxhat1, S.dx, 0, S.sp1.ns, S.sp1.nh, sums1, cnt1)
     del dxhat1
-    dxhat0, sums0, cnt0 = _spade_conv_bwd(G, blk, S.sp0, blk.conv_0, inv_of, ddx, 3, 1, seg4, seg_cache)
+    dxhat0, sums0, cnt0 = _spade_conv_bwd(G, blk, S.sp0, blk.conv_0, inv_of, ddx, 3, 1, seg4)
     del ddx
     dx = ops.bn_bwd_apply(dxhat0, S.x, S.xs, S.sp0.ns, S.sp0.nh, sums0, cnt0)
     del dxhat0
     if blk.learned_shortcut:
-        dxhat_s, sums_s, cnt_s = _spade_conv_bwd(G, blk, S.sps, blk.conv_s, inv_of, dy, 1, 0, seg4, seg_cache)
+        dxhat_s, sums_s, cnt_s = _spade_conv_bwd(G, blk, S.sps, blk.conv_s, inv_of, dy, 1, 0, seg4)
         ops.bn_bwd_apply(dxhat_s, S.x, S.xs, S.sps.ns, S.sps.nh, sums_s, cnt_s, dx=dx)
     else:
         ops.bn_bwd_apply(dy, S.x, S.xs, None, None, None, 1, dx=dx)   # identity shortcut through the upsample
@@ -173,8 +160,7 @@ def fc_bwd(G, fc, S, dout):
         dy = ops.in_bwd(da, L.y_in, L.ss, _LRELU, pmul=L.pm_in)
     dz = ops.act_bwd(dy, None, _NONE, pm1=S.l1.upd, pm2=S.l1.ratio)
     G.add(fc.layer1.bias, ops.chan_sum(ops.act_bwd(dy, None, _NONE, pm1=S.l1.upd)))
-    dwt1 = (ops.thin_wgrad_tc(ops.pad_channels32(S.x0), dz, 3, 3, 2, 1, 4) if ops.thin_wgrad_tc_enabled()
-            else ops.thin_wgrad(S.x0, dz, 3, 3, 2, 1))
+    dwt1 = ops.thin_wgrad(S.x0, dz, 3, 3, 2, 1)
     G.add(fc.layer1.weight, _thin_wt_to_oihw(dwt1, 3, 3, 3))
 
 
@@ -191,8 +177,7 @@ def bg_bwd(G, bg, S, dfeats):
         d = ops.reflect_pad_bwd(dxp, 1, dx=d_list[i])
     dz0 = ops.act_bwd(d, S.x0, _RELU)
     G.add(bg.conv1.conv.bias, ops.chan_sum(dz0))
-    dwt1 = (ops.thin_wgrad_tc(ops.pad_channels32(S.inp, reflect_pad=3), dz0, 7, 7, 1, 0, 4) if ops.thin_wgrad_tc_enabled()
-            else ops.thin_wgrad(S.inp, dz0, 7, 7, 1, 3, pad_mode=1))
+    dwt1 = ops.thin_wgrad(S.inp, dz0, 7, 7, 1, 3, pad_mode=1)
     G.add(bg.conv1.conv.weight, _thin_wt_to_oihw(dwt1, 7, 7, 3))
 
 
@@ -270,8 +255,7 @@ def _d_scale_bwd(G, D, S, douts, inv_of, need_dimg, param_grads):
     conv0 = D.model0[0]
     dz0 = ops.act_bwd(df, S.f0, _LRELU)
     if param_grads:
-        dwt0 = (ops.thin_wgrad_tc(ops.pad_channels32(S.x8), dz0, 4, 4, 2, D.padw, 8) if ops.thin_wgrad_tc_enabled()
-                else ops.thin_wgrad(S.x8, dz0, 4, 4, 2, D.padw))
+        dwt0 = ops.thin_wgrad(S.x8, dz0, 4, 4, 2, D.padw)
         G.add(conv0.weight, _thin_wt_to_oihw(dwt0, 4, 4, conv0.weight.shape[1]))
         G.add(conv0.bias, ops.chan_sum(dz0))
     if not need_dimg:

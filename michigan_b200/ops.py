@@ -6,8 +6,6 @@ libmichigan_sm90.so.  Activations are NHWC fp32 ([N,H,W,C] contiguous).
 import ctypes as C
 import math
 
-import os
-
 import torch
 
 from . import _lib
@@ -58,9 +56,6 @@ def _chk(t, name, dtype=torch.float32):
 
 # widest GEMM N tile of the implicit-GEMM kernels (128 accumulator columns per consumer warpgroup)
 _SPADE_BN_MAX = 128
-# N tile of split-precision 3x3 / stride-1 convs routed to the M-tile-group kernel (0 = the launcher's default: min(Cout, 128)).
-# 64: merged accumulators of 128 columns for every such layer
-_CONV3_BN = int(os.environ.get("MG_CONV3_BN", "0"))
 
 
 def spade_bn(c):
@@ -145,9 +140,6 @@ def conv_igemm(x, wpack, cout, kh, kw, stride=1, pad=0, *, act=ACT_NONE, round_o
     a.N, a.H, a.W, a.Cin = N, H, W, Cin
     a.OH, a.OW, a.Cout = OH, OW, cout
     a.KH, a.KW, a.stride, a.pad = kh, kw, stride, pad
-    if bn == 0 and _CONV3_BN and spade is None and x_lo is not None and kh == 3 and kw == 3 and stride == 1 and pad == 1 \
-            and OW % 16 == 0 and OH >= 16 and cout > _CONV3_BN and cout % _CONV3_BN == 0:
-        bn = _CONV3_BN
     a.BN = bn
     a.epi = EPI_SPADE if spade is not None else EPI_BIAS
     a.act, a.round_out = act, int(round_out)
@@ -244,14 +236,9 @@ def conv_seg_tc(seg4, wpack, bias, *, seg_resize=0, act=ACT_RELU, round_out=Fals
     return out
 
 
-def seg_tc_enabled():
-    """MG_SEG_TC=0 falls back to the direct fp32 kernel (thin_conv) for SPADE's mlp_shared."""
-    return os.environ.get("MG_SEG_TC", "1") != "0"
-
-
 def pack_mlp_shared(w_oihw):
     """Operand of SPADE's mlp_shared conv (label_nc <= 4 -> 128, 3x3): tensor-core bf16 split, or the thin-conv layout."""
-    if seg_tc_enabled() and w_oihw.shape[0] == 128 and w_oihw.shape[1] <= 4:
+    if w_oihw.shape[0] == 128 and w_oihw.shape[1] <= 4:
         return pack_weight_seg_tc(w_oihw)
     return pack_weight_thin(w_oihw, 4)
 
@@ -809,30 +796,6 @@ def in_bwd(df, x, ss, act=ACT_LRELU, pmul=None, round_tf32=False):
     check(_lib.load().mg_in_bwd(_p(df), _p(x), _p(ss), _p(sums), _p(dx), N, H * W, Cc, act, _p(pmul), int(round_tf32), _stream()),
           "mg_in_bwd")
     return dx
-
-
-def pad_channels32(x, seg_resize=0, in_hw=None, reflect_pad=0):
-    """[N,H,W,CinP] -> TF32-rounded [N,H+2p,W+2p,32] (zero channel pad, optional nearest resize / reflect pad)."""
-    _chk(x, "x")
-    N = x.shape[0]
-    H, W = in_hw if seg_resize else (x.shape[1], x.shape[2])
-    out = torch.empty((N, H + 2 * reflect_pad, W + 2 * reflect_pad, 32), device=x.device, dtype=torch.float32)
-    check(_lib.load().mg_pad_channels32(_p(x), _p(out), N, H, W, x.shape[-1], seg_resize, reflect_pad, _stream()), "mg_pad_channels32")
-    return out
-
-
-def thin_wgrad_tc_enabled():
-    """MG_THIN_WGRAD_TC=1 routes the thin-conv weight gradients through the tensor-core wgrad on 32-padded channels
-    (N = 32 MMAs sit on the ~100-cycle issue floor); default is the register-tiled CUDA-core kernel (mg_thin_wgrad)."""
-    return os.environ.get("MG_THIN_WGRAD_TC", "0") == "1"
-
-
-def thin_wgrad_tc(x32, dz, kh, kw, stride, pad, cinp):
-    """Weight gradient of a thin conv on the tensor cores: x32 from pad_channels32 (already reflect-padded when the
-    conv uses reflection padding: pass pad=0 then).  Returns the thin layout [kh*kw][cinp][Cout]."""
-    cout = dz.shape[-1]
-    dwp = conv_wgrad(dz, x32, kh, kw, stride, pad)               # [Cout][kh*kw*32]
-    return dwp.view(cout, kh * kw, 32)[:, :, :cinp].permute(1, 2, 0).contiguous()
 
 
 def thin_wgrad(x, dz, kh, kw, stride, pad, pad_mode=0, seg_resize=0, in_hw=None, relu_src=None, want_bias=False):

@@ -31,11 +31,11 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), "symbol %s declared in the header but not exported" % name
 
 
-def test_ctypes_signatures_cover_the_header():
+def test_ctypes_signatures_and_abi_version_match_the_header():
     from michigan_b200 import _lib
     assert sorted(_lib.SIGNATURES) == declared_functions()
     lib = _lib.load()
-    assert lib.mg_version() == 2
+    assert lib.mg_version() == 3
     assert lib.mg_launch_count() >= 0
 
 
@@ -80,16 +80,19 @@ def test_ops_refuse_cpu_tensors():
         ops.pack_weight(torch.zeros(32, 32, 3, 3))
 
 
-def test_schedule_knobs_named_in_the_header_exist():
-    """Every schedule knob the header documents is known to mg_get_tuning / mg_set_tuning (host-only calls); unknown names fail."""
+def test_header_knobs_exist_and_retired_knobs_are_rejected():
+    """Every schedule knob the header documents is known to mg_get_tuning / mg_set_tuning (host-only calls); unknown names fail,
+    and so do the retired names of knobs that had no effect on sm_90a."""
     import re
     from michigan_b200 import _lib
     lib = _lib.load()
     text = open(os.path.join(ROOT, "include", "michigan_b200.h")).read()
     names = sorted(set(re.findall(r'"(MG_[A-Z0-9_]+)"', text)))
-    assert {"MG_DUAL", "MG_GROUP3", "MG_SEG_TMA", "MG_WGRAD_HALO", "MG_EPI_TMA"} <= set(names)
+    assert {"MG_GROUP3", "MG_SEG_TMA", "MG_EPI_REG", "MG_MERGE"} <= set(names)
     for n in names:
         v = lib.mg_get_tuning(n.encode())
         assert v > -(1 << 30), n
         assert lib.mg_set_tuning(n.encode(), v) == 0, n
     assert lib.mg_set_tuning(b"MG_NO_SUCH_KNOB", 1) < 0
+    for n in ("MG_DUAL", "MG_WGRAD_DUAL", "MG_WGRAD_HALO", "MG_EPI_TMA", "MG_EPI_EARLY"):
+        assert lib.mg_set_tuning(n.encode(), 1) == -2, n

@@ -93,36 +93,28 @@ def test_igemm_16bit_operands(gen, N, h, Cin, Cout, k, s, p):
 
 
 @pytest.mark.parametrize("fmt", ["tf32", "bf3"])
-def test_igemm_dual_pipelines(gen, fmt):
+def test_igemm_persistent_ctas_several_tiles(gen, fmt):
     """Persistent CTAs with several tiles each: max_ctas=3 gives 5 and 6 tiles per CTA (odd and even) through one stage ring
-    and one accumulator tile.  MG_DUAL has no effect on sm_90a, so both runs take the same path: only the comparison with the
-    fp32 conv2d is meaningful."""
+    and one accumulator tile."""
     ops = _ops()
     N, h, Cin, Cout = 2, 32, 64, 64
     x = torch.randn(N, Cin, h, h, generator=gen).to(dev)
     w = (torch.randn(Cout, Cin, 3, 3, generator=gen) / 24).to(dev)
     b = torch.randn(Cout, generator=gen).to(dev)
-    outs = {}
-    for dual in ("1", "0"):
-        prev_knob = _lib_mod().set_tuning("MG_DUAL", int(dual))
-        try:
-            if fmt == "tf32":
-                xt, wt = tf32_trunc(x), tf32_trunc(w)
-                ref = F.conv2d(xt, wt, b, padding=1)
-                outs[dual] = ops.conv_igemm(nhwc(xt), ops.pack_weight(wt, None, round_tf32=True), Cout, 3, 3, 1, 1, bias=b, max_ctas=3)
-                tol = 2e-5
-            else:
-                xn = nhwc(x)
-                hi = xn.bfloat16()
-                lo = (xn - hi.float()).bfloat16()
-                ref = F.conv2d(x, w, b, padding=1)
-                outs[dual] = ops.conv_igemm(hi, ops.pack_weight16(w, None, ops.BF16, split=True), Cout, 3, 3, 1, 1, bias=b, a_fmt=ops.BF16,
-                                            x_lo=lo, max_ctas=3)
-                tol = 6e-5
-        finally:
-            _lib_mod().set_tuning("MG_DUAL", prev_knob)
-        assert rel_err(nchw(outs[dual]), ref) <= tol, dual
-    assert torch.equal(outs["1"], outs["0"])   # same MMA order per output tile -> bit-identical
+    if fmt == "tf32":
+        xt, wt = tf32_trunc(x), tf32_trunc(w)
+        ref = F.conv2d(xt, wt, b, padding=1)
+        out = ops.conv_igemm(nhwc(xt), ops.pack_weight(wt, None, round_tf32=True), Cout, 3, 3, 1, 1, bias=b, max_ctas=3)
+        tol = 2e-5
+    else:
+        xn = nhwc(x)
+        hi = xn.bfloat16()
+        lo = (xn - hi.float()).bfloat16()
+        ref = F.conv2d(x, w, b, padding=1)
+        out = ops.conv_igemm(hi, ops.pack_weight16(w, None, ops.BF16, split=True), Cout, 3, 3, 1, 1, bias=b, a_fmt=ops.BF16,
+                             x_lo=lo, max_ctas=3)
+        tol = 6e-5
+    assert rel_err(nchw(out), ref) <= tol
 
 
 def test_igemm_halo_mode_matches_classic(gen):
@@ -169,7 +161,7 @@ def test_fused_spade_epilogue(gen, N, h, C, xs):
 @pytest.mark.parametrize("N,H,W,R,cin", [(2, 32, 32, 1, 4), (1, 64, 64, 4, 4), (3, 16, 16, 2, 4), (2, 24, 40, 1, 3), (2, 18, 9, 4, 4)])
 def test_seg_conv_tensor_core(gen, N, H, W, R, cin):
     """SPADE mlp_shared (normalization.py:92-96,110-111) as one K=128 bf16-split GEMM vs fp32 conv: 3e-5; the direct
-    fp32 kernel (MG_SEG_TC=0 route) must agree as well."""
+    fp32 kernel (mlp_shared's thin-layout operand) must agree as well."""
     ops = _ops()
     seg = torch.randn(N, 4, H * R, W * R, generator=gen).to(dev)
     seg[:, cin:] = 0
@@ -257,7 +249,7 @@ def test_tensor_core_wgrad_and_dgrad(gen, N, h, Cin, Cout, k, s, p):
 
 @pytest.mark.parametrize("N,h,Cin,Cout,k,s,p", [(2, 32, 64, 64, 3, 1, 1), (2, 40, 128, 256, 3, 1, 1), (2, 33, 64, 128, 4, 2, 2), (3, 8, 128, 64, 1, 1, 0),
                                                    (2, 33, 256, 128, 4, 1, 2), (1, 20, 64, 64, 3, 1, 1)])
-def test_wgrad_bf16_operands(gen, N, h, Cin, Cout, k, s, p):
+def test_wgrad_bf16_operands_vs_autograd(gen, N, h, Cin, Cout, k, s, p):
     """The weight-gradient GEMM with bf16 operands (MN-major, plain 128B swizzle, K = 16 pixels per MMA) against torch autograd on
     bf16-exact operands (fp32 accumulation on both sides)."""
     ops = _ops()
@@ -266,15 +258,9 @@ def test_wgrad_bf16_operands(gen, N, h, Cin, Cout, k, s, p):
     y = F.conv2d(x, w, None, stride=s, padding=p)
     dy = torch.randn(y.shape, generator=gen).to(dev).bfloat16().float()
     y.backward(dy)
-    from michigan_b200 import _lib
-    for halo in (0, 1):      # 1 (default): stride-1 layers load ONE input patch per stage, the KW taps read shifted views of it
-        prev = _lib.set_tuning("MG_WGRAD_HALO", halo)
-        try:
-            dwp = ops.conv_wgrad16(nhwc(dy).bfloat16(), nhwc(x.detach()).bfloat16(), k, k, s, p)
-            dw = ops.unpack_wgrad(dwp, tuple(w.shape))
-        finally:
-            _lib.set_tuning("MG_WGRAD_HALO", prev)
-        assert rel_err(dw, w.grad) <= 5e-5, halo
+    dwp = ops.conv_wgrad16(nhwc(dy).bfloat16(), nhwc(x.detach()).bfloat16(), k, k, s, p)
+    dw = ops.unpack_wgrad(dwp, tuple(w.shape))
+    assert rel_err(dw, w.grad) <= 5e-5
     assert torch.equal(ops.cvt16(nhwc(dy)), nhwc(dy).bfloat16())
     sums, d16 = ops.chan_sum_cvt16(nhwc(dy))
     assert torch.equal(d16, nhwc(dy).bfloat16())
@@ -282,37 +268,29 @@ def test_wgrad_bf16_operands(gen, N, h, Cin, Cout, k, s, p):
 
 
 @pytest.mark.parametrize("fmt", ["tf32", "f16", "bf3"])
-def test_igemm_dual_pipelines_n256(gen, fmt):
-    """Same as test_igemm_dual_pipelines for a 256-column GEMM N (two 128-column tiles); again only the fp32 comparison is
-    meaningful."""
+def test_igemm_persistent_ctas_several_tiles_n256(gen, fmt):
+    """Same as test_igemm_persistent_ctas_several_tiles for a 256-column GEMM N (two 128-column tiles)."""
     ops = _ops()
     N, h, Cin, Cout = 2, 32, 64, 256
     x = torch.randn(N, Cin, h, h, generator=gen).to(dev)
     w = (torch.randn(Cout, Cin, 3, 3, generator=gen) / 24).to(dev)
     b = torch.randn(Cout, generator=gen).to(dev)
-    outs = {}
-    for dual in ("2", "0"):
-        prev_knob = _lib_mod().set_tuning("MG_DUAL", int(dual))
-        try:
-            if fmt == "tf32":
-                xt, wt = tf32_trunc(x), tf32_trunc(w)
-                ref, tol = F.conv2d(xt, wt, b, padding=1), 2e-5
-                outs[dual] = ops.conv_igemm(nhwc(xt), ops.pack_weight(wt, None, round_tf32=True), Cout, 3, 3, 1, 1, bias=b, max_ctas=3)
-            elif fmt == "f16":
-                ref, tol = F.conv2d(x.half().float(), w.half().float(), b, padding=1), 2e-5
-                outs[dual] = ops.conv_igemm(nhwc(x).half(), ops.pack_weight16(w, None, ops.F16, split=False), Cout, 3, 3, 1, 1, bias=b,
-                                            a_fmt=ops.F16, max_ctas=3)
-            else:
-                xn = nhwc(x)
-                hi = xn.bfloat16()
-                lo = (xn - hi.float()).bfloat16()
-                ref, tol = F.conv2d(x, w, b, padding=1), 6e-5
-                outs[dual] = ops.conv_igemm(hi, ops.pack_weight16(w, None, ops.BF16, split=True), Cout, 3, 3, 1, 1, bias=b, a_fmt=ops.BF16,
-                                            x_lo=lo, max_ctas=3)
-        finally:
-            _lib_mod().set_tuning("MG_DUAL", prev_knob)
-        assert rel_err(nchw(outs[dual]), ref) <= tol, dual
-    assert torch.equal(outs["2"], outs["0"])
+    if fmt == "tf32":
+        xt, wt = tf32_trunc(x), tf32_trunc(w)
+        ref, tol = F.conv2d(xt, wt, b, padding=1), 2e-5
+        out = ops.conv_igemm(nhwc(xt), ops.pack_weight(wt, None, round_tf32=True), Cout, 3, 3, 1, 1, bias=b, max_ctas=3)
+    elif fmt == "f16":
+        ref, tol = F.conv2d(x.half().float(), w.half().float(), b, padding=1), 2e-5
+        out = ops.conv_igemm(nhwc(x).half(), ops.pack_weight16(w, None, ops.F16, split=False), Cout, 3, 3, 1, 1, bias=b,
+                             a_fmt=ops.F16, max_ctas=3)
+    else:
+        xn = nhwc(x)
+        hi = xn.bfloat16()
+        lo = (xn - hi.float()).bfloat16()
+        ref, tol = F.conv2d(x, w, b, padding=1), 6e-5
+        out = ops.conv_igemm(hi, ops.pack_weight16(w, None, ops.BF16, split=True), Cout, 3, 3, 1, 1, bias=b, a_fmt=ops.BF16,
+                             x_lo=lo, max_ctas=3)
+    assert rel_err(nchw(out), ref) <= tol
 
 
 def test_fused_loss_reductions_vs_reference_formulas(gen):
@@ -441,10 +419,9 @@ def test_conv3x3_group_kernel_spade_epilogue(gen):
 
 
 @pytest.mark.parametrize("N,h,w,C,xsh,act", [(2, 32, 32, 128, 1, 2), (1, 24, 40, 128, 0, 0), (2, 16, 48, 256, 1, 2)])
-def test_spade_epilogue_tma_store(gen, N, h, w, C, xsh, act):
+def test_spade_epilogue_bf16_hi_lo_operand(gen, N, h, w, C, xsh, act):
     """SPADE gamma|beta GEMM -> bf16 hi/lo operand (the SPEC 1/2 epilogue specialisations) against the fp32 formula; ragged tiles
-    (24 x 40) exercise the edge masking.  MG_EPI_TMA has no effect on sm_90a: both settings take the same path, so only the
-    fp32 comparison is meaningful."""
+    (24 x 40) exercise the edge masking."""
     ops = _ops()
     actv = torch.randn(N, h, w, 128, generator=gen).to(dev)
     wg = (torch.randn(C, 128, 3, 3, generator=gen) / 34).to(dev)
@@ -452,16 +429,9 @@ def test_spade_epilogue_tma_store(gen, N, h, w, C, xsh, act):
     xs = torch.randn(N, h >> xsh, w >> xsh, C, generator=gen).to(dev)
     ns, nh, g1, bb = [torch.randn(C, generator=gen).to(dev) for _ in range(4)]
     wp = ops.pack_weight_gb16(wg, wb)
-    outs = {}
-    for knob in (2, 1, 0):      # 2 = 1 + L1 prefetch of x ahead of the accumulator wait
-        prev = _lib_mod().set_tuning("MG_EPI_TMA", knob)
-        try:
-            _, hi, lo = ops.conv_igemm(actv.half(), wp, C, 3, 3, 1, 1, act=act, a_fmt=ops.F16, spade=(xs, xsh, ns, nh, g1, bb),
-                                       out16=(ops.BF16, True), want_f32=False, max_ctas=3)
-            torch.cuda.synchronize()
-            outs[knob] = hi.float() + lo.float()
-        finally:
-            _lib_mod().set_tuning("MG_EPI_TMA", prev)
+    _, hi, lo = ops.conv_igemm(actv.half(), wp, C, 3, 3, 1, 1, act=act, a_fmt=ops.F16, spade=(xs, xsh, ns, nh, g1, bb),
+                               out16=(ops.BF16, True), want_f32=False, max_ctas=3)
+    out = hi.float() + lo.float()
     a16 = nchw(actv.half().float())
     gamma = F.conv2d(a16, wg.half().float(), None, padding=1)
     beta = F.conv2d(a16, wb.half().float(), None, padding=1)
@@ -470,9 +440,7 @@ def test_spade_epilogue_tma_store(gen, N, h, w, C, xsh, act):
     ref = xh * (g1.view(1, -1, 1, 1) + gamma) + (bb.view(1, -1, 1, 1) + beta)
     if act == 2:
         ref = F.leaky_relu(ref, 0.2)
-    assert rel_err(nchw(outs[1]), ref) <= 1e-4 and rel_err(nchw(outs[0]), ref) <= 1e-4
-    assert torch.equal(outs[2], outs[1])
-    assert rel_err(outs[1], outs[0]) <= 2e-5      # hi + lo carries 16 significand bits; the two epilogues contract their FMAs differently
+    assert rel_err(nchw(out), ref) <= 1e-4
 
 
 @pytest.mark.parametrize("N,H,W,Cin", [(2, 32, 64, 64), (1, 20, 45, 64), (1, 9, 33, 32)])

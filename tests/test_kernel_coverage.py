@@ -21,7 +21,6 @@ NOT_IN_GPU_TESTS = {
     "mg_peer_allreduce_f64": "needs two GPUs: tests/nccl_worker.py runs it on 2 GPUs (launched by test_gpu_multi.py)",
     "mg_peer_buffer_bytes": "size query of the 2-GPU all-reduce, called by tests/nccl_worker.py on 2 GPUs",
     "mg_peer_max_elems": "size query of the 2-GPU all-reduce, called by tests/nccl_worker.py on 2 GPUs",
-    "mg_debug_igemm_prof": "probe counters, compiled only into the -DMG_PROBES build that tools/ load",
     "mg_debug_seg_prof": "probe counters, compiled only into the -DMG_PROBES build that tools/ load",
     "mg_version": "ABI query, checked by tests/test_abi.py",
     "mg_launch_count": "ABI query, checked by tests/test_abi.py",
@@ -238,7 +237,7 @@ def test_ops_wrappers_call_declared_entry_points():
     assert not undeclared, undeclared
 
 
-def test_every_entry_point_is_exercised_by_a_gpu_test():
+def test_every_header_entry_point_is_exercised_by_a_gpu_test():
     eps = entry_points()
     reach = exercised_by_gpu_tests()
     assert set(NOT_IN_GPU_TESTS) <= eps, sorted(set(NOT_IN_GPU_TESTS) - eps)

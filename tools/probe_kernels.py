@@ -489,11 +489,6 @@ def group_bwd2():
         dw = dwt.view(k, k, CinP, Cout).permute(3, 2, 0, 1)[:, :Cin]
         torch.cuda.synchronize()
         report("thin_wgrad %d->%d k%d s%d pm%d" % (Cin, Cout, k, s_, pmode), dw, w.grad, 2e-5)
-        x32 = ops.pad_channels32(ops.nchw_to_nhwc(x.detach(), CinP), reflect_pad=p_ if pmode else 0)
-        dwt2 = ops.thin_wgrad_tc(x32, nhwc(dz), k, k, s_, 0 if pmode else p_, CinP)
-        dw2 = dwt2.view(k, k, CinP, Cout).permute(3, 2, 0, 1)[:, :Cin]
-        torch.cuda.synchronize()
-        report("thin_wgrad_tc %d->%d k%d s%d pm%d (tf32)" % (Cin, Cout, k, s_, pmode), dw2, w.grad, 2e-3)
         if Cin == 7:
             dimg = torch.zeros(2, 3, 32, 32, device=dev)
             ops.thin_dgrad3(nhwc(dz), ops.pack_weight_thin(w.detach(), 8), dimg, k, k, s_, p_, 4)
@@ -506,9 +501,7 @@ def group_bwd2():
     y.backward(dz)
     dwt = ops.thin_wgrad(nhwc(seg), nhwc(dz), 3, 3, 1, 1, seg_resize=4, in_hw=(16, 16))
     report("thin_wgrad seg_resize", dwt.view(3, 3, 4, 128).permute(3, 2, 0, 1), w.grad, 2e-5)
-    dwt2 = ops.thin_wgrad_tc(ops.pad_channels32(nhwc(seg), seg_resize=4, in_hw=(16, 16)), nhwc(dz), 3, 3, 1, 1, 4)
-    report("thin_wgrad_tc seg_resize (tf32)", dwt2.view(3, 3, 4, 128).permute(3, 2, 0, 1), w.grad, 2e-3)
-    # timing at the training shapes: register-tiled CUDA-core kernel vs the tensor-core route on 32-padded channels
+    # timing at the training shapes
     for label, cinp, cout, k, s_, p_, pm, S_, Nn in (("bg conv1 3->64 k7 reflect 8x512^2", 4, 64, 7, 1, 3, 1, 512, 8),
                                                     ("D model0 7->64 k4 s2 16x512^2", 8, 64, 4, 2, 2, 0, 512, 16),
                                                     ("mlp_shared 4->128 k3 8x512^2", 4, 128, 3, 1, 1, 0, 512, 8)):
@@ -516,8 +509,7 @@ def group_bwd2():
         oh = (S_ + 2 * p_ - k) // s_ + 1
         dzz = torch.randn(Nn, oh, oh, cout, device=dev)
         t_new = _time(lambda: ops.thin_wgrad(xin, dzz, k, k, s_, p_, pad_mode=pm))
-        t_tc = _time(lambda: ops.thin_wgrad_tc(ops.pad_channels32(xin, reflect_pad=p_) if pm else ops.pad_channels32(xin), dzz, k, k, s_, 0 if pm else p_, cinp))
-        print("perf thin wgrad %-36s register-tiled %.3f ms, tensor-core(32-padded, incl. pad) %.3f ms" % (label, t_new, t_tc), flush=True)
+        print("perf thin wgrad %-36s register-tiled %.3f ms" % (label, t_new), flush=True)
         del xin, dzz
     # ---- conv_img backward
     x = torch.randn(2, 64, 24, 40, generator=g).to(dev).requires_grad_(True)
