@@ -323,19 +323,28 @@ int mg_orient_rgb(const float* orient, const float* label, float* out_nchw, int 
 int mg_hole_mask(const float* mask, const float* orient_mask, const float* th_u, const float* idx_u, float* hole, int N, int H, int W,
                  void* stream);
 
-/* ---- adversarial loss reductions (models/networks/loss.py:19-140 GANLoss hinge, 144-175 GANFeatLoss) ------------------
+/* ---- adversarial loss reductions (models/networks/loss.py:19-140 GANLoss, every gan_mode, 144-175 GANFeatLoss) ----------
  * mg_edge_weight: the wide-edge weight map of one discriminator scale (loss.py:60-78): label [N,H,W] (hair mask, 0/1)
  * -> out [N,h,w] = edges*wide_edge + (1-edges), edges = nearest-resized (maxpool_k - minpool_k) of the nearest-resized
  * label, k = max(1, int(0.06*h)), pad k/2 (pooled maps are h+1 wide for even k, resized back as the reference does). */
 int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, int w, float wide_edge, void* stream);
 /* One launch for all terms of a loss evaluation.  terms_dev: device array of n_terms records of mg_loss_term_bytes()
- * bytes each, layout {const float* a; const float* b; float* ga; long long n; float scale, sign; int op, out_slot;}:
+ * bytes each, layout {const float* a; const float* b; float* ga; long long n; float scale, sign; int op, out_slot;
+ * float target; int den_slot; const float* label; long long label_ns; int C, h, w, H, W, channels_last;}:
  *   slots[out_slot] += scale * sum_i f(a_i, b_i)   (fp64 accumulation; caller zeroes `slots`)
  *   op 0: f = min(sign*a - 1, 0) * (b ? b_i : 1)   hinge, discriminator side (b = weight map)     loss.py:104-120
- *   op 1: f = a                                    generator hinge -mean(D(fake))                  loss.py:123-124
+ *   op 1: f = a                                    generator hinge -mean(D(fake)), gan_mode 'w'     loss.py:123-124
  *   op 2: f = |a - b|                              feature matching, b detached                    loss.py:170-172
  *   op 3: f = (a - b)^2                            content loss (MSE of relu5_1), b detached       loss.py:662-666
- * mg_loss_reduce_bwd writes ga_i = gslots[out_slot] * scale * df/da for every term with ga != null. */
+ *   op 4: f = BCE-with-logits(a, target)           gan_mode 'original'                              loss.py:81-84
+ *   op 5: f = (a - target)^2                       gan_mode 'ls'                                   loss.py:85-87
+ * ops 6-8 (--remove_background) read l = label[n, 0] at a's element [n, c, y, x] (a is [N,C,h,w], NCHW or, channels_last,
+ * NHWC) through the nearest resize of the [N,1,H,W] label to (h, w), and add l over a's elements into slots[den_slot]:
+ *   op 6: f = a l                                  generator hinge                                  loss.py:117
+ *   op 7: f = min((sign*a - 1) l, 0)               discriminator hinge                              loss.py:110-114
+ *   op 8: f = |a l - b l|                          masked feature matching, b detached              loss.py:154-161
+ * mg_loss_reduce_bwd writes ga_i = gslots[out_slot] * scale * df/da for every term with ga != null (torch's tie rules: the
+ * binary min gives each side half, |.| has gradient 0 at 0; BCE: sigmoid(a) - target). */
 int mg_loss_reduce(const void* terms_dev, int n_terms, double* slots, void* stream);
 int mg_loss_reduce_bwd(const void* terms_dev, int n_terms, const float* gslots, void* stream);
 int mg_loss_term_bytes(void);

@@ -4,13 +4,28 @@
 // (models/networks/loss.py:60-78,100-140: interpolate -> 2x max_pool2d -> interpolate -> clamp -> mul -> mean;
 // loss.py:163-175: 8x l1_loss), ~60 launches per iteration forward and as many backward.  Here:
 //   * mg_edge_weight      the wide-edge weight map of one discriminator scale (loss.py:60-78) in one kernel;
-//   * mg_loss_reduce      ALL terms of a loss evaluation (hinge terms of every scale, the eight feature-matching L1 terms)
-//                         through one descriptor table: warp-shuffle + fp64 atomics into the loss slots;
+//   * mg_loss_reduce      ALL terms of a loss evaluation (the GAN terms of every scale in every gan_mode, the eight
+//                         feature-matching L1 terms, masked or not) through one descriptor table: warp-shuffle + fp64 atomics
+//                         into the loss slots;
 //   * mg_loss_reduce_bwd  the matching gradients, one launch for every tensor in the table.
 #include <cuda_runtime.h>
 #include "mg_internal.h"
 
 namespace mg {
+
+// torch's nearest source index (F.interpolate mode='nearest', upsample_nearest2d): floor(dst * (in / out)) in fp32, clamped to
+// the last row / column.  scale = (float)in / (float)out.
+__device__ __forceinline__ int nearest_src(int dst, float scale, int in) {
+    const int s = (int)floorf(dst * scale);
+    return s < in - 1 ? s : in - 1;
+}
+
+// label[n, 0, i', j'] of an [N,1,H,W] label read at (i, j) of its nearest resize to (h, w), sh = H / h, sw = W / w; rows of
+// W contiguous floats, image n at n * ns (the hair channel of the one-hot label map is read in place, ns = C * H * W).
+__device__ __forceinline__ float label_nearest(const float* __restrict__ label, long long ns, int n, int i, int j, int H, int W,
+                                               float sh, float sw) {
+    return __ldg(label + n * ns + (long long)nearest_src(i, sh, H) * W + nearest_src(j, sw, W));
+}
 
 // loss.py:60-66 get_wide_edges on the nearest-resized label + loss.py:73-78 weight = edges*wide_edge + (1-edges).
 //   t[i,j]      = label[floor(i*H/h), floor(j*W/w)]                       (F.interpolate, mode nearest)
@@ -28,18 +43,15 @@ __global__ void edge_weight_kernel(const float* __restrict__ label, float* __res
         const int j = (int)(idx % w);
         const int i = (int)((idx / w) % h);
         const int n = (int)(idx / ((long long)w * h));
-        int a = (int)floorf(i * ph), b = (int)floorf(j * pw);
-        a = a < hp - 1 ? a : hp - 1; b = b < wp - 1 ? b : wp - 1;
+        const int a = nearest_src(i, ph, hp), b = nearest_src(j, pw, wp);
         float mx = -1e30f, mn = 1e30f;
         for (int di = 0; di < k; ++di) {
             const int ti = a - p + di;
             if (ti < 0 || ti >= h) continue;
-            int si = (int)floorf(ti * sh); si = si < H - 1 ? si : H - 1;
             for (int dj = 0; dj < k; ++dj) {
                 const int tj = b - p + dj;
                 if (tj < 0 || tj >= w) continue;
-                int sj = (int)floorf(tj * sw); sj = sj < W - 1 ? sj : W - 1;
-                const float v = __ldg(label + ((size_t)n * H + si) * W + sj);
+                const float v = label_nearest(label, (long long)H * W, n, ti, tj, H, W, sh, sw);
                 mx = fmaxf(mx, v); mn = fminf(mn, v);
             }
         }
@@ -53,13 +65,27 @@ __global__ void edge_weight_kernel(const float* __restrict__ label, float* __res
 //   op 1  plain sum: f = a                                                    (generator hinge: -mean(D(fake)), loss.py:123-124)
 //   op 2  L1: f = |a - b|                                                     (GANFeatLoss, loss.py:170-172; b is detached)
 //   op 3  squared difference: f = (a - b)^2                                   (content loss, loss.py:662-666; b is detached)
+//   op 4  BCE with logits against the constant t: f = (1 - t) a + max(-a, 0) + log1p(exp(-|a|))   (gan_mode 'original', loss.py:81-84)
+//   op 5  squared error against the constant t: f = (a - t)^2                 (gan_mode 'ls', loss.py:85-87)
+// The masked ops read l = the [N,1,H,W] hair label at a's element through the nearest resize to (h, w) (loss.py:107, 157), and
+// also add l over a's elements into slots[den_slot] (= sum(label1) * c, the caller divides):
+//   op 6  weighted sum: f = a l                                               (generator hinge, --remove_background, loss.py:117)
+//   op 7  masked hinge: f = min((sign*a - 1) l, 0)                            (discriminator hinge, --remove_background, 110-114)
+//   op 8  masked L1: f = |a l - b l|                                          (GANFeatLoss.L1_loss_mask, loss.py:154-161)
 struct LossTerm {
     const float* a;
-    const float* b;      // op 0: weight map (nullable); op 2: the other tensor
+    const float* b;      // op 0: weight map (nullable); ops 2, 3, 8: the other tensor
     float* ga;           // backward: gradient w.r.t. a (written, not accumulated); null = skip
     long long n;
     float scale, sign;
     int op, out_slot;
+    // appended for ops 4-8 (zero for ops 0-3)
+    float target;        // ops 4, 5
+    int den_slot;        // ops 6-8
+    const float* label;  // ops 6-8: [N,1,H,W], rows contiguous, image n at label + n * label_ns
+    long long label_ns;
+    int C, h, w, H, W;   // ops 6-8: a is [N,C,h,w]; the label's spatial size
+    int channels_last;   // ops 6-8: a (and b) laid out NHWC (the discriminator's permuted views), else NCHW
 };
 
 // grid.x blocks per term: terms range from 9 K (coarse logits) to 34 M elements (finest feature map) - enough blocks to saturate
@@ -69,10 +95,81 @@ constexpr int kLossBlocksPerTerm = 592;
 // (a - b)^2 with the square rounded before it is summed (no fused multiply-add across terms)
 __device__ __forceinline__ float sq_diff(float a, float b) { const float d = a - b; return __fmul_rn(d, d); }
 
+// l of element i of a masked term (ops 6-8): a's index -> (n, y, x) in NCHW or NHWC order, then the label's nearest lookup
+__device__ __forceinline__ float term_label(const LossTerm& t, long long i, float sh, float sw) {
+    const long long chw = (long long)t.C * t.h * t.w;
+    const int n = (int)(i / chw);
+    const int r = (int)(i - n * chw);
+    const int p = t.channels_last ? r / t.C : r % (t.h * t.w);
+    return label_nearest(t.label, t.label_ns, n, p / t.w, p % t.w, t.H, t.W, sh, sw);
+}
+
+// f of ops 4-8 at element i (l = the element's label for ops 6-8)
+__device__ __forceinline__ float term_f(const LossTerm& t, float a, long long i, float l) {
+    switch (t.op) {
+    case 4: return __fmul_rn(1.f - t.target, a) + fmaxf(-a, 0.f) + log1pf(expf(-fabsf(a)));
+    case 5: return sq_diff(a, t.target);
+    case 6: return __fmul_rn(a, l);
+    case 7: return fminf(__fmul_rn(t.sign * a - 1.f, l), 0.f);
+    default: return fabsf(__fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l));
+    }
+}
+
+// df/da of ops 4-8; ties as torch: the binary min gives each side half, |.| has gradient 0 at 0
+__device__ __forceinline__ float term_df(const LossTerm& t, float a, long long i, float l) {
+    switch (t.op) {
+    case 4: {
+        const float e = expf(-fabsf(a));
+        const float sig = a >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+        return sig - t.target;
+    }
+    case 5: return 2.f * (a - t.target);
+    case 6: return l;
+    case 7: {
+        const float m = __fmul_rn(t.sign * a - 1.f, l);
+        return m < 0.f ? t.sign * l : (m == 0.f ? 0.5f * t.sign * l : 0.f);
+    }
+    default: {
+        const float df = __fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l);
+        return df > 0.f ? l : (df < 0.f ? -l : 0.f);
+    }
+    }
+}
+
+// block-wide fp64 sum of one value per thread (256 threads); the result is valid in thread 0
+__device__ __forceinline__ double block_sum(double acc, double* part) {
+    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    double s = 0.0;
+    if (threadIdx.x == 0)
+        for (int i = 0; i < 8; ++i) s += part[i];
+    return s;
+}
+
 __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __restrict__ terms, double* __restrict__ slots) {
     const LossTerm t = terms[blockIdx.y];
     if ((long long)blockIdx.x * blockDim.x >= t.n && blockIdx.x != 0) return;      // no element of this term falls to this block
+    __shared__ double part[8];
     float accf = 0.f;
+    if (t.op >= 4) {
+        // ops 4-8: one element per thread per trip, fp32 partials per thread, fp64 across threads
+        const bool masked = t.op >= 6;
+        const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;
+        float accl = 0.f;
+        for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
+            const float l = masked ? term_label(t, i, sh, sw) : 0.f;
+            accf += term_f(t, __ldg(t.a + i), i, l);
+            accl += l;
+        }
+        const double s = block_sum((double)accf, part);
+        if (threadIdx.x == 0) atomicAdd(slots + t.out_slot, s * (double)t.scale);
+        if (!masked) return;
+        __syncthreads();
+        const double sl = block_sum((double)accl, part);
+        if (threadIdx.x == 0) atomicAdd(slots + t.den_slot, sl);
+        return;
+    }
     // 4 elements per thread per trip (float4 when the term is 16-byte aligned), fp32 partials per thread, fp64 across threads
     const bool vec = ((reinterpret_cast<uintptr_t>(t.a) | reinterpret_cast<uintptr_t>(t.b)) & 15) == 0;
     const long long n4 = vec ? t.n / 4 : 0;
@@ -92,25 +189,26 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
         else if (t.op == 2) accf += fabsf(a - __ldg(t.b + i));
         else accf += sq_diff(a, __ldg(t.b + i));
     }
-    double acc = (double)accf;
-    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
-    __shared__ double part[8];
-    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int i = 0; i < 8; ++i) s += part[i];
-        atomicAdd(slots + t.out_slot, s * (double)t.scale);
-    }
+    const double s = block_sum((double)accf, part);
+    if (threadIdx.x == 0) atomicAdd(slots + t.out_slot, s * (double)t.scale);
 }
 
 // ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * ([sign*a - 1 < 0] + [sign*a - 1 == 0] / 2);  op 1: 1;
-// op 2: sgn(a - b);  op 3: 2 (a - b).  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0)) gives each side
-// half the gradient.
+// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-8: term_df.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
+// gives each side half the gradient.  The masked ops' denominators are folded into gslot by the caller.
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
     const LossTerm t = terms[blockIdx.y];
     if (!t.ga) return;
     const float g = __ldg(gslots + t.out_slot) * t.scale;
+    if (t.op >= 4) {
+        const bool masked = t.op >= 6;
+        const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;
+        for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
+            const float l = masked ? term_label(t, i, sh, sw) : 0.f;
+            t.ga[i] = g * term_df(t, __ldg(t.a + i), i, l);
+        }
+        return;
+    }
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
         const float a = __ldg(t.a + i);
         float d;

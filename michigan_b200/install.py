@@ -59,12 +59,13 @@ def install(reference_root=None, compat=True):
                  "patch_replication_callback", "convert_model", "patch_sync_batchnorm"):
         setattr(sbn, name, getattr(mine.sync_batchnorm, name))
     pkg.SPADEBGenerator, pkg.MultiscaleDiscriminator, pkg.NLayerDiscriminator = G, MSD, NLD
-    # the perceptual, style / content, background and Lab colour losses (pix2pix_model.py:41-53 look them up as networks.VGGLoss,
+    # the GAN and GAN feature-matching losses (pix2pix_model.py:36-39, networks.GANLoss, networks.GANFeatLoss), the perceptual,
+    # style / content, background and Lab colour losses (pix2pix_model.py:41-53 look them up as networks.VGGLoss,
     # networks.StyleContentLoss, networks.RGBBackgroundL1Loss, networks.LabColorLoss) and the hair-average Lab loss of the
     # unpaired stage (pix2pix_model.py:55-56, networks.HairAvgLabLoss).  The rgb term is a bare nn.L1Loss (pix2pix_model.py:51)
     # and stays torch's: torch.nn is not patched.
     los = importlib.import_module("models.networks.loss")
-    for name in ("VGGLoss", "StyleContentLoss", "RGBBackgroundL1Loss", "LabColorLoss", "HairAvgLabLoss"):
+    for name in ("GANLoss", "GANFeatLoss", "VGGLoss", "StyleContentLoss", "RGBBackgroundL1Loss", "LabColorLoss", "HairAvgLabLoss"):
         setattr(los, name, getattr(mine.loss, name))
         setattr(pkg, name, getattr(mine.loss, name))
     if getattr(gen, "InpaintGenerator", None) is not None:

@@ -7,7 +7,7 @@ from .base_network import BaseNetwork
 from .normalization import SPADE, get_nonspade_norm_layer
 from .architecture import SPADEResnetBlock, VGG19
 from . import loss
-from .loss import VGGLoss, LabColorLoss, StyleContentLoss, RGBBackgroundL1Loss, HairAvgLabLoss
+from .loss import GANLoss, GANFeatLoss, VGGLoss, LabColorLoss, StyleContentLoss, RGBBackgroundL1Loss, HairAvgLabLoss
 from .encoder import ImageEncoder3, BackgroundEncode2, PartialConv2d, ConvBlock
 from .generator import SPADEBGenerator
 from .discriminator import MultiscaleDiscriminator, NLayerDiscriminator

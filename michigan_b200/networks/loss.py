@@ -1,6 +1,6 @@
-"""Hinge GAN loss and GAN feature-matching loss with the reference's call signatures
-(models/networks/loss.py:19-140 `GANLoss`, 144-175 `GANFeatLoss`; in-scope modes: gan_mode='hinge',
-remove_background=False), evaluated by the fused reduction kernels of csrc/mg_loss.cu:
+"""GAN loss and GAN feature-matching loss with the reference's call signatures
+(models/networks/loss.py:19-140 `GANLoss`, every gan_mode ('ls', 'original', 'w', 'hinge'), 144-175 `GANFeatLoss`, with and
+without --remove_background), evaluated by the fused reduction kernels of csrc/mg_loss.cu:
 
   * every call = ONE forward launch (all discriminator scales / all eight feature terms through a descriptor table,
     fp64 accumulation) and ONE backward launch, instead of ~10 eager ops per scale and per term;
@@ -10,6 +10,7 @@ The rest of the generator objective follows: the Gabor orientation loss, VGGLoss
 pass, _VGGObjectiveFn), LabColorLoss, RGBBackgroundL1Loss and the rgb L1 (RGBL1Loss).
 """
 import ctypes as C
+from collections import namedtuple
 
 import torch
 import torch.nn as nn
@@ -19,11 +20,28 @@ from .. import _lib, ops
 
 class _Term(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("ga", C.c_void_p), ("n", C.c_longlong), ("scale", C.c_float),
-                ("sign", C.c_float), ("op", C.c_int32), ("out_slot", C.c_int32)]
+                ("sign", C.c_float), ("op", C.c_int32), ("out_slot", C.c_int32),
+                # appended for ops 4-8 (zero for ops 0-3)
+                ("target", C.c_float), ("den_slot", C.c_int32), ("label", C.c_void_p), ("label_ns", C.c_longlong),
+                ("C", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+                ("channels_last", C.c_int32)]
 
 
 OP_HINGE_D, OP_SUM, OP_L1, OP_SQ = 0, 1, 2, 3
+# gan_mode 'original' / 'ls' against a constant target; the --remove_background terms, masked by the resized hair label
+OP_BCE, OP_SQ_T, OP_WSUM, OP_HINGE_MASK, OP_L1_MASK = 4, 5, 6, 7, 8
+MASKED_OPS = (OP_WSUM, OP_HINGE_MASK, OP_L1_MASK)
+DEN_EPS = 1e-5          # loss.py:111, 114, 117, 160: sum(label1) * c + 1e-5
 _table_cache = {}
+
+
+class _Spec(namedtuple("_Spec", "op ai b scale sign slot target label")):
+    """One loss term: op, index of its differentiable input `a`, the detached `b` (or None), scale, hinge sign, output slot;
+    the constant target of ops 4 and 5; the [N,1,H,W] hair label of the masked ops."""
+    __slots__ = ()
+
+    def __new__(cls, op, ai, b, scale, sign, slot, target=0.0, label=None):
+        return super().__new__(cls, op, ai, b, scale, sign, slot, target, label)
 
 
 def _dense(t):
@@ -31,6 +49,21 @@ def _dense(t):
     if t.is_contiguous() or (t.dim() == 4 and t.is_contiguous(memory_format=torch.channels_last)):
         return t
     return t.contiguous()
+
+
+def _hair_label(label, x):
+    """The [N,1,H,W] label the masked terms of x ([N,C,h,w]) read in place: fp32, rows contiguous, any image stride (the hair
+    channel of the one-hot label map is a view)."""
+    if label is None:
+        raise ValueError("--remove_background needs the hair label")
+    lab = label.detach()
+    if lab.dim() != 4 or lab.shape[1] != 1 or lab.shape[0] != x.shape[0] or x.dim() != 4:
+        raise ValueError("--remove_background: label %s does not match the [N,C,h,w] input %s" % (tuple(lab.shape), tuple(x.shape)))
+    lab = lab.float()
+    _, _, H, W = lab.shape
+    if not ((W == 1 or lab.stride(3) == 1) and (H == 1 or lab.stride(2) == W)):
+        lab = lab.contiguous()
+    return lab
 
 
 def _device_table(terms, device):
@@ -46,29 +79,63 @@ def _device_table(terms, device):
     return buf
 
 
+def _term(s, a, b, ga, out_slot, den_slot):
+    t = _Term(a.data_ptr(), b.data_ptr() if b is not None else None, ga, a.numel(), float(s.scale), float(s.sign), s.op, out_slot)
+    t.target = float(s.target)
+    if s.op in MASKED_OPS:
+        lab = s.label
+        t.den_slot, t.label, t.label_ns = den_slot, lab.data_ptr(), lab.stride(0)
+        t.C, t.h, t.w = a.shape[1], a.shape[2], a.shape[3]
+        t.H, t.W = lab.shape[2], lab.shape[3]
+        t.channels_last = int(not a.is_contiguous())
+    return t
+
+
 class _LossFn(torch.autograd.Function):
-    """spec: list of (op, a_index, b_tensor_or_None, scale, sign, slot); tensors: the differentiable `a` inputs."""
+    """spec: list of _Spec (or of their first six fields as a tuple); tensors: the differentiable `a` inputs.  A masked term k (ops 6-8) sums into a slot of its own,
+    nslots + k', and its label sum into nslots + m + k' (m masked terms); its slot then adds num / (den + 1e-5) on the
+    device, and its gradient is scaled by the same 1 / (den + 1e-5)."""
 
     @staticmethod
     def forward(ctx, spec, nslots, *tensors):
         assert _lib.load().mg_loss_term_bytes() == C.sizeof(_Term)
+        spec = [s if isinstance(s, _Spec) else _Spec(*s) for s in spec]        # plain (op, ai, b, scale, sign, slot) tuples too
         dense = [_dense(t.detach()) for t in tensors]
         dev = dense[0].device
+        masked = [k for k, s in enumerate(spec) if s.op in MASKED_OPS]
+        m = len(masked)
+        if m and len({spec[k].slot for k in masked}) != 1:
+            raise ValueError("the masked terms of one loss add into one slot")
         terms = []
         keep = []
-        for op, ai, b, scale, sign, slot in spec:
-            a = dense[ai]
-            bb = _dense(b.detach()) if b is not None else None
+        slot_of = {}
+        for k, s in enumerate(spec):
+            a = dense[s.ai]
+            bb = _dense(s.b.detach()) if s.b is not None else None
             if bb is not None:
                 assert bb.numel() == a.numel(), (bb.shape, a.shape)
+                if s.op == OP_L1_MASK:
+                    assert bb.shape == a.shape and bb.stride() == a.stride(), (bb.shape, bb.stride(), a.shape, a.stride())
                 keep.append(bb)
-            terms.append(_Term(a.data_ptr(), bb.data_ptr() if bb is not None else None, None, a.numel(), float(scale), float(sign), op, slot))
-        slots = torch.zeros(nslots, device=dev, dtype=torch.float64)
+            out_slot, den_slot = s.slot, 0
+            if s.op in MASKED_OPS:
+                j = masked.index(k)
+                out_slot, den_slot = nslots + j, nslots + m + j
+                assert a.dim() == 4 and s.label.shape[0] == a.shape[0]
+            slot_of[k] = (out_slot, den_slot)
+            terms.append(_term(s, a, bb, None, out_slot, den_slot))
+        slots = torch.zeros(nslots + 2 * m, device=dev, dtype=torch.float64)
         table = _device_table(terms, dev)
         _lib.check(_lib.load().mg_loss_reduce(table.data_ptr(), len(terms), slots.data_ptr(), ops._stream()), "mg_loss_reduce")
-        ctx.spec, ctx.dense, ctx.keep, ctx.nslots = spec, dense, keep, nslots
+        ctx.spec, ctx.dense, ctx.keep, ctx.nslots, ctx.slot_of, ctx.inv = spec, dense, keep, nslots, slot_of, None
         ctx.shapes = [(t.shape, t.stride(), d.stride()) for t, d in zip(tensors, dense)]
-        return slots.float()
+        if not m:
+            return slots.float()
+        # loss.py:111, 114, 117, 160: each masked term divided by its own sum(label1) * c + 1e-5, on the device
+        ctx.inv = 1.0 / (slots[nslots + m:] + DEN_EPS)
+        out = slots[:nslots].clone()
+        out[spec[masked[0]].slot] += (slots[nslots:nslots + m] * ctx.inv).sum()
+        return out.float()
 
     @staticmethod
     def backward(ctx, gslots):
@@ -83,15 +150,17 @@ class _LossFn(torch.autograd.Function):
         flat = torch.empty(total, device=dev, dtype=torch.float32)
         seen = set()
         terms = []
-        for (op, ai, b, scale, sign, slot), kb in zip(ctx.spec, _iter_keep(ctx.spec, ctx.keep)):
-            if ai in seen:
+        for k, (s, kb) in enumerate(zip(ctx.spec, _iter_keep(ctx.spec, ctx.keep))):
+            if s.ai in seen:
                 raise RuntimeError("a tensor may appear in one loss term only")
-            seen.add(ai)
-            a = dense[ai]
-            terms.append(_Term(a.data_ptr(), kb.data_ptr() if kb is not None else None, flat.data_ptr() + 4 * offs[ai], a.numel(),
-                               float(scale), float(sign), op, slot))
+            seen.add(s.ai)
+            terms.append(_term(s, dense[s.ai], kb, flat.data_ptr() + 4 * offs[s.ai], *ctx.slot_of[k]))
         table = _device_table(terms, dev)
         g = gslots.contiguous().float()
+        if ctx.inv is not None:
+            m = ctx.inv.numel()
+            slot = next(s.slot for s in ctx.spec if s.op in MASKED_OPS)
+            g = torch.cat([g, (g[slot].double() * ctx.inv).float(), torch.zeros(m, device=dev, dtype=torch.float32)])
         _lib.check(_lib.load().mg_loss_reduce_bwd(table.data_ptr(), len(terms), g.data_ptr(), ops._stream()), "mg_loss_reduce_bwd")
         grads = []
         for i, (shape, stride, dstride) in enumerate(ctx.shapes):
@@ -104,18 +173,25 @@ class _LossFn(torch.autograd.Function):
 
 def _iter_keep(spec, keep):
     it = iter(keep)
-    for op, ai, b, scale, sign, slot in spec:
-        yield next(it) if b is not None else None
+    for s in spec:
+        yield next(it) if s.b is not None else None
+
+
+GAN_MODES = ("ls", "original", "w", "hinge")
 
 
 class GANLoss(nn.Module):
+    """loss.py:19-140 for every gan_mode: 'original' BCE with logits and 'ls' MSE against target_real_label /
+    target_fake_label, 'w' -+mean, 'hinge' with the wide-edge weight map (wide_edge > 1) or, under --remove_background, the
+    hair-masked terms over sum(label1) * c + 1e-5.  The mean of each scale, averaged over the discriminators."""
+
     def __init__(self, gan_mode, target_real_label=1.0, target_fake_label=0.0, tensor=torch.FloatTensor, opt=None):
         super().__init__()
-        if gan_mode != "hinge":
-            raise NotImplementedError("michigan_b200: gan_mode '%s' (only 'hinge' is on the hot path)" % gan_mode)
-        if getattr(opt, "remove_background", False):
-            raise NotImplementedError("michigan_b200: --remove_background is not implemented")
+        if gan_mode not in GAN_MODES:
+            raise ValueError("Unexpected gan_mode {}".format(gan_mode))
         self.gan_mode = gan_mode
+        self.real_label = target_real_label
+        self.fake_label = target_fake_label
         self.opt = opt
         self._wcache = {}
 
@@ -136,20 +212,33 @@ class GANLoss(nn.Module):
         self._wcache[key] = out
         return out
 
+    def _term(self, i, x, num, target_is_real, for_discriminator, label):
+        """The _Spec of one scale's loss (loss.py:80-124) over num discriminators."""
+        inv = 1.0 / (x.numel() * num)
+        if self.gan_mode in ("original", "ls"):
+            target = self.real_label if target_is_real else self.fake_label
+            return _Spec(OP_BCE if self.gan_mode == "original" else OP_SQ_T, i, None, inv, 1.0, 0, target=target)
+        if self.gan_mode == "w":
+            return _Spec(OP_SUM, i, None, -inv if target_is_real else inv, 1.0, 0)
+        if getattr(self.opt, "remove_background", False):
+            lab = _hair_label(label, x)
+            if for_discriminator:
+                return _Spec(OP_HINGE_MASK, i, None, -1.0 / num, 1.0 if target_is_real else -1.0, 0, label=lab)
+            assert target_is_real, "The generator's hinge loss must be aiming for real"
+            return _Spec(OP_WSUM, i, None, -1.0 / num, 1.0, 0, label=lab)
+        if for_discriminator:
+            wmap = self.get_weight_mask(x, label) if self.opt.wide_edge > 1.0 else None
+            return _Spec(OP_HINGE_D, i, wmap, -1.0 / (x.numel() * num), 1.0 if target_is_real else -1.0, 0)
+        assert target_is_real, "The generator's hinge loss must be aiming for real"
+        return _Spec(OP_SUM, i, None, -1.0 / (x.numel() * num), 1.0, 0)
+
     def __call__(self, input, target_is_real, for_discriminator=True, label=None):
         """loss.py:126-140: list over discriminators (each possibly a list of features, the logits last) -> mean over
         discriminators of the per-scale loss, a [1] tensor."""
         preds = input if isinstance(input, list) else [input]
         logits = [(p[-1] if isinstance(p, list) else p) for p in preds]
         num = len(logits)
-        spec = []
-        for i, x in enumerate(logits):
-            if for_discriminator:
-                wmap = self.get_weight_mask(x, label) if self.opt.wide_edge > 1.0 else None
-                spec.append((OP_HINGE_D, i, wmap, -1.0 / (x.numel() * num), 1.0 if target_is_real else -1.0, 0))
-            else:
-                assert target_is_real, "The generator's hinge loss must be aiming for real"
-                spec.append((OP_SUM, i, None, -1.0 / (x.numel() * num), 1.0, 0))
+        spec = [self._term(i, x, num, target_is_real, for_discriminator, label) for i, x in enumerate(logits)]
         return _LossFn.apply(spec, 1, *logits)
 
 
@@ -159,8 +248,10 @@ class GANFeatLoss(nn.Module):
         self.opt = opt
 
     def forward(self, pred_fake, pred_real, label=None):
-        """loss.py:163-175: sum over discriminators and their intermediate features of L1(fake, real.detach()) * lambda_feat / num_D."""
+        """loss.py:163-175: sum over discriminators and their intermediate features of L1(fake, real.detach()) * lambda_feat / num_D;
+        under --remove_background the hair-masked L1_loss_mask (loss.py:154-161), each term over its own sum(label1) * c + 1e-5."""
         num_D = len(pred_fake)
+        lab = _hair_label(label, pred_fake[0][0]) if getattr(self.opt, "remove_background", False) else None
         spec, tensors = [], []
         for i in range(num_D):
             for j in range(len(pred_fake[i]) - 1):
@@ -170,7 +261,10 @@ class GANFeatLoss(nn.Module):
                 if fd.stride() != rd.stride():
                     rd = r.contiguous()
                     fd = f.contiguous()
-                spec.append((OP_L1, len(tensors), rd, self.opt.lambda_feat / (num_D * f.numel()), 1.0, 0))
+                if lab is not None:
+                    spec.append(_Spec(OP_L1_MASK, len(tensors), rd, self.opt.lambda_feat / num_D, 1.0, 0, label=lab))
+                else:
+                    spec.append(_Spec(OP_L1, len(tensors), rd, self.opt.lambda_feat / (num_D * f.numel()), 1.0, 0))
                 tensors.append(fd)
         return _LossFn.apply(spec, 1, *tensors)
 

@@ -1,7 +1,7 @@
 """Pix2PixModel — the mode-dispatching caller of the hot path, mirroring the reference's
 models/pix2pix_model.py (forward 62-122, create_optimizers 124-152, preprocess_input 209-254,
 compute_generator_loss 257-365, compute_discriminator_loss 367-398, generate_fake 505-541,
-discriminate 546-594) for the in-scope configuration: netG=spadeb, netD=multiscale, hinge GAN loss +
+discriminate 546-594) for the in-scope configuration: netG=spadeb, netD=multiscale, the GAN loss of any --gan_mode +
 GAN feature loss and, each behind its --no_* flag, every other term of the reference's curr_step-1 objective (VGG
 perceptual, style / content, background and rgb L1, Lab colour, Gabor orientation / confidence).  With the reference checkout
 present, `michigan_b200.install()` lets the reference's own Pix2PixModel/Pix2PixTrainer drive these networks instead (INTEGRATION.md); this class is the
@@ -31,9 +31,10 @@ class Pix2PixModel(torch.nn.Module):
         for flag in ("use_vae", "use_blender", "use_instance_feat", "unpairTrain"):
             if getattr(opt, flag, False):
                 raise NotImplementedError("michigan_b200: --%s is outside the hot path (SURVEY.md §8)" % flag)
-        # Every term of the reference's generator objective for curr_step 1 (pix2pix_model.py:296-345) is computed here: hinge
-        # GAN, GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT, CONFIDENCE, each dropped by its --no_* flag.
-        # --remove_background and --balance_Lab are refused by the loss classes.
+        # Every term of the reference's generator objective for curr_step 1 (pix2pix_model.py:296-345) is computed here: GAN
+        # (any --gan_mode), GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT, CONFIDENCE, each dropped by its --no_*
+        # flag.  GANLoss and GANFeatLoss take --remove_background; VGGLoss and StyleContentLoss refuse it, and LabColorLoss
+        # refuses --balance_Lab.
         self.netIG = None
         if getattr(opt, "use_ig", False):
             self.netIG = networks.define_IG(opt)
