@@ -330,7 +330,7 @@ int mg_hole_mask(const float* mask, const float* orient_mask, const float* th_u,
 int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, int w, float wide_edge, void* stream);
 /* One launch for all terms of a loss evaluation.  terms_dev: device array of n_terms records of mg_loss_term_bytes()
  * bytes each, layout {const float* a; const float* b; float* ga; long long n; float scale, sign; int op, out_slot;
- * float target; int den_slot; const float* label; long long label_ns; int C, h, w, H, W, channels_last;}:
+ * float target; int den_slot; const float* label; long long label_ns; int C, h, w, H, W, channels_last; const float* add;}:
  *   slots[out_slot] += scale * sum_i f(a_i, b_i)   (fp64 accumulation; caller zeroes `slots`)
  *   op 0: f = min(sign*a - 1, 0) * (b ? b_i : 1)   hinge, discriminator side (b = weight map)     loss.py:104-120
  *   op 1: f = a                                    generator hinge -mean(D(fake)), gan_mode 'w'     loss.py:123-124
@@ -338,13 +338,19 @@ int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, i
  *   op 3: f = (a - b)^2                            content loss (MSE of relu5_1), b detached       loss.py:662-666
  *   op 4: f = BCE-with-logits(a, target)           gan_mode 'original'                              loss.py:81-84
  *   op 5: f = (a - target)^2                       gan_mode 'ls'                                   loss.py:85-87
- * ops 6-8 (--remove_background) read l = label[n, 0] at a's element [n, c, y, x] (a is [N,C,h,w], NCHW or, channels_last,
- * NHWC) through the nearest resize of the [N,1,H,W] label to (h, w), and add l over a's elements into slots[den_slot]:
+ * ops 6-10 (--remove_background) read l = label[n, 0] at a's element [n, c, y, x] (a is [N,C,h,w], NCHW or, channels_last,
+ * NHWC) through the nearest resize of the [N,1,H,W] label to (h, w); ops 6-9 add l over a's elements into slots[den_slot]:
  *   op 6: f = a l                                  generator hinge                                  loss.py:117
  *   op 7: f = min((sign*a - 1) l, 0)               discriminator hinge                              loss.py:110-114
- *   op 8: f = |a l - b l|                          masked feature matching, b detached              loss.py:154-161
- * mg_loss_reduce_bwd writes ga_i = gslots[out_slot] * scale * df/da for every term with ga != null (torch's tie rules: the
- * binary min gives each side half, |.| has gradient 0 at 0; BCE: sigmoid(a) - target). */
+ *   op 8: f = |a l - b l|                          masked feature matching / VGG L1, b detached     loss.py:154-161, 187-196
+ *   op 9: f = (a l - b l)^2                        masked content loss, b detached                  loss.py:664-677
+ *   op 10: masked channel moments (calc_mean_std_mask, loss.py:634-654), l binary: per (n, c) slots[out_slot + n*2C + c] +=
+ *          sum l a and slots[out_slot + n*2C + C + c] += sum l a^2 (mg_in_stats' [N][2][C] layout, fp32 runs of at most 32
+ *          elements, fp64 above; scale not applied), and per image slots[den_slot + n] += sum l over its pixels (once per pixel).
+ * mg_loss_reduce_bwd writes ga_i = add_i + gslots[out_slot] * scale * df/da for every term with ga != null (add null: ga_i =
+ * gslots[out_slot] * scale * df/da; add may alias ga; no two terms of one launch may write the same ga).  Torch's tie rules:
+ * the binary min gives each side half, |.| has gradient 0 at 0; BCE: sigmoid(a) - target.  Op 9: df/da = 2 (a l - b l) l.
+ * Op 10: b is the [N][3][C] fp32 table (mu', A, B) of mg_style_loss_fwd's masked mode, df/da = l (A + B (a - mu')). */
 int mg_loss_reduce(const void* terms_dev, int n_terms, double* slots, void* stream);
 int mg_loss_reduce_bwd(const void* terms_dev, int n_terms, const float* gslots, void* stream);
 int mg_loss_term_bytes(void);
@@ -405,16 +411,21 @@ int mg_hair_avg_lab_fwd(const float* fake_nchw, const float* real_nchw, const fl
 int mg_hair_avg_lab_bwd(const float* fake_nchw, const float* mask_fake, const double* sums, const float* gscale, float* dfake_nchw,
                         int N, int H, int W, void* stream);
 
-/* ---- style and content losses (models/networks/loss.py:624-711 StyleContentLoss with remove_background = False) ----------
+/* ---- style and content losses (models/networks/loss.py:624-711 StyleContentLoss) -------------------------------------------
  * Replaces calc_mean_std (loss.py:624-632), calc_style_loss and calc_content_loss (loss.py:662-683) over the five VGG19 taps.
  * The per-(n, c) statistics are mg_in_stats' fp64 sums ([N][2][C]: sum x, sum x^2) of each fp32 NHWC tap, one call per tap over
  * the whole fake || target batch; the content loss is op 3 of mg_loss_reduce.
  * mg_style_loss_fwd: taps_host: HOST array of n_taps (<= 8) records of mg_style_tap_bytes() bytes, layout
- *   {const double* sums_f; const double* sums_t; float* coef; long long M; int N, C;}  (M = pixels per image, C % 4 == 0).
+ *   {const double* sums_f; const double* sums_t; float* coef; long long M; int N, C; const double* cnt_f; const double* cnt_t;}
+ *   (M = pixels per image, C % 4 == 0).
  *   mu = S1 / M, sigma = sqrt((S2 - S1 mu) / (M - 1) + 1e-5) (unbiased variance, as torch.var); in fp64:
  *   loss[0] += sum over taps of (sum_nc (mu_f - mu_t)^2 + (sigma_f - sigma_t)^2) / (N*C)   (caller zeroes; one block, so the
  *   sum is bit-reproducible); coef [N][3][C] (16-byte aligned) = fp32 mu_f, mu_f - mu_t, (sigma_f - sigma_t) / sigma_f.
  *   A tap with M < 2 (relu5_1 of a crop below 32) is refused with -2; the reference returns NaN there.
+ *   Masked mode (--remove_background; cnt_f, cnt_t both set, null = unmasked): S1, S2 are mg_loss_reduce op 10's sums and cnt
+ *   its per-image mask sums D ([N] each), the mask binary: mu = S1 / (D + eps), sigma = sqrt((S2 - mu (2 S1 - mu D)) / (D + eps)
+ *   + eps), eps = 1e-5 (calc_mean_std_mask: biased, eps twice; no pixel-count refusal); coef = op 10's backward table
+ *   mu_f (1 + eps / (D_f + eps)), 2 (mu_f - mu_t) / (N C (D_f + eps)), 2 (sigma_f - sigma_t) / (N C sigma_f (D_f + eps)).
  * mg_style_tap_grad: gradient w.r.t. one fake tap x [N, HW, C] (fp32 NHWC, C % 4 == 0, 16-byte aligned), g = device [2] floats
  *   (upstream gradients of the style and content losses):
  *   out = add + g[0] (2 (mu_f - mu_t) / (N C HW) + 2 (sigma_f - sigma_t) / (N C sigma_f (HW - 1)) (x - mu_f))

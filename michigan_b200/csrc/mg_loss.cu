@@ -71,7 +71,14 @@ __global__ void edge_weight_kernel(const float* __restrict__ label, float* __res
 // also add l over a's elements into slots[den_slot] (= sum(label1) * c, the caller divides):
 //   op 6  weighted sum: f = a l                                               (generator hinge, --remove_background, loss.py:117)
 //   op 7  masked hinge: f = min((sign*a - 1) l, 0)                            (discriminator hinge, --remove_background, 110-114)
-//   op 8  masked L1: f = |a l - b l|                                          (GANFeatLoss.L1_loss_mask, loss.py:154-161)
+//   op 8  masked L1: f = |a l - b l|                                          (GANFeatLoss.L1_loss_mask, loss.py:154-161;
+//                                                                             VGGLoss.L1_loss_mask, loss.py:187-196)
+//   op 9  masked squared difference: f = (a l - b l)^2                       (calc_content_loss, loss.py:664-677)
+//   op 10 masked channel moments of a (NHWC or NCHW): for every (n, c), slots[out_slot + n*2C + c] += sum l a and
+//         slots[out_slot + n*2C + C + c] += sum l a^2 (mg_in_stats' [N][2][C] layout; scale is not applied), and
+//         slots[den_slot + n] += sum l over the image's PIXELS (each pixel once, not once per channel)    (calc_mean_std_mask,
+//         loss.py:634-654).  Backward: b is a [N][3][C] fp32 table (mu', A, B) written by mg_style_loss_fwd's masked mode and
+//         f'(a) = l (A + B (a - mu')).  The labels are binary (a channel of the one-hot label map, nearest-resized), l^2 = l.
 struct LossTerm {
     const float* a;
     const float* b;      // op 0: weight map (nullable); ops 2, 3, 8: the other tensor
@@ -85,7 +92,10 @@ struct LossTerm {
     const float* label;  // ops 6-8: [N,1,H,W], rows contiguous, image n at label + n * label_ns
     long long label_ns;
     int C, h, w, H, W;   // ops 6-8: a is [N,C,h,w]; the label's spatial size
-    int channels_last;   // ops 6-8: a (and b) laid out NHWC (the discriminator's permuted views), else NCHW
+    int channels_last;   // ops 6-10: a (and b) laid out NHWC (the discriminator's permuted views, the VGG taps), else NCHW
+    // appended for the accumulating backward (null for every term before it)
+    const float* add;    // backward: ga = add + g f'(a) (may alias ga); null: ga = g f'(a).  No two terms of one launch may
+                         // write the same ga.
 };
 
 // grid.x blocks per term: terms range from 9 K (coarse logits) to 34 M elements (finest feature map) - enough blocks to saturate
@@ -95,7 +105,7 @@ constexpr int kLossBlocksPerTerm = 592;
 // (a - b)^2 with the square rounded before it is summed (no fused multiply-add across terms)
 __device__ __forceinline__ float sq_diff(float a, float b) { const float d = a - b; return __fmul_rn(d, d); }
 
-// l of element i of a masked term (ops 6-8): a's index -> (n, y, x) in NCHW or NHWC order, then the label's nearest lookup
+// l of element i of a masked term (ops 6-10): a's index -> (n, y, x) in NCHW or NHWC order, then the label's nearest lookup
 __device__ __forceinline__ float term_label(const LossTerm& t, long long i, float sh, float sw) {
     const long long chw = (long long)t.C * t.h * t.w;
     const int n = (int)(i / chw);
@@ -104,18 +114,24 @@ __device__ __forceinline__ float term_label(const LossTerm& t, long long i, floa
     return label_nearest(t.label, t.label_ns, n, p / t.w, p % t.w, t.H, t.W, sh, sw);
 }
 
-// f of ops 4-8 at element i (l = the element's label for ops 6-8)
+// channel of element i of a masked term
+__device__ __forceinline__ int term_channel(const LossTerm& t, long long i) {
+    return (int)(t.channels_last ? i % t.C : (i / ((long long)t.h * t.w)) % t.C);
+}
+
+// f of ops 4-9 at element i (l = the element's label for ops 6-9)
 __device__ __forceinline__ float term_f(const LossTerm& t, float a, long long i, float l) {
     switch (t.op) {
     case 4: return __fmul_rn(1.f - t.target, a) + fmaxf(-a, 0.f) + log1pf(expf(-fabsf(a)));
     case 5: return sq_diff(a, t.target);
     case 6: return __fmul_rn(a, l);
     case 7: return fminf(__fmul_rn(t.sign * a - 1.f, l), 0.f);
+    case 9: return sq_diff(__fmul_rn(a, l), __fmul_rn(__ldg(t.b + i), l));
     default: return fabsf(__fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l));
     }
 }
 
-// df/da of ops 4-8; ties as torch: the binary min gives each side half, |.| has gradient 0 at 0
+// df/da of ops 4-10; ties as torch: the binary min gives each side half, |.| has gradient 0 at 0
 __device__ __forceinline__ float term_df(const LossTerm& t, float a, long long i, float l) {
     switch (t.op) {
     case 4: {
@@ -129,10 +145,52 @@ __device__ __forceinline__ float term_df(const LossTerm& t, float a, long long i
         const float m = __fmul_rn(t.sign * a - 1.f, l);
         return m < 0.f ? t.sign * l : (m == 0.f ? 0.5f * t.sign * l : 0.f);
     }
+    case 9: return 2.f * (__fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l)) * l;
+    case 10: {
+        const int n = (int)(i / ((long long)t.C * t.h * t.w)), c = term_channel(t, i);
+        const float* co = t.b + (size_t)n * 3 * t.C + c;
+        return l * (__ldg(co + t.C) + __ldg(co + 2 * t.C) * (a - __ldg(co)));
+    }
     default: {
         const float df = __fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l);
         return df > 0.f ? l : (df < 0.f ? -l : 0.f);
     }
+    }
+}
+
+// op 10: each thread adds l a and l a^2 of its elements in fp32 runs of at most 32, carries the runs in fp64 and flushes them
+// into the (n, c) slots whenever its (n, c) changes.  The grid stride (kLossBlocksPerTerm x 256 = 2^12 x 37) is a multiple of
+// every VGG channel count, so an NHWC thread keeps one channel and flushes once per image.
+__device__ __noinline__ void moments_term(const LossTerm& t, double* __restrict__ slots) {
+    const float sh = (float)t.H / (float)t.h, sw = (float)t.W / (float)t.w;
+    const long long chw = (long long)t.C * t.h * t.w, stride = (long long)gridDim.x * blockDim.x;
+    long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    int cn = -1, cc = 0, run = 0;
+    float f1 = 0.f, f2 = 0.f, fl = 0.f;
+    double d1 = 0.0, d2 = 0.0, dl = 0.0;
+    for (;; i += stride) {
+        const bool more = i < t.n;
+        const int n = more ? (int)(i / chw) : -2, c = more ? term_channel(t, i) : 0;
+        if (n != cn || c != cc || run == 32) {
+            d1 += (double)f1; d2 += (double)f2; dl += (double)fl;
+            f1 = f2 = fl = 0.f;
+            run = 0;
+            if ((n != cn || c != cc) && cn >= 0) {
+                double* s = slots + t.out_slot + (size_t)cn * 2 * t.C + cc;
+                if (d1 != 0.0) atomicAdd(s, d1);
+                if (d2 != 0.0) atomicAdd(s + t.C, d2);
+                if (dl != 0.0) atomicAdd(slots + t.den_slot + cn, dl);
+                d1 = d2 = dl = 0.0;
+            }
+            cn = n; cc = c;
+        }
+        if (!more) break;
+        const float l = term_label(t, i, sh, sw), a = __ldg(t.a + i);
+        const float la = __fmul_rn(a, l);
+        f1 += la;
+        f2 += __fmul_rn(la, a);
+        if (c == 0) fl += l;
+        ++run;
     }
 }
 
@@ -152,8 +210,12 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
     if ((long long)blockIdx.x * blockDim.x >= t.n && blockIdx.x != 0) return;      // no element of this term falls to this block
     __shared__ double part[8];
     float accf = 0.f;
+    if (t.op == 10) {
+        moments_term(t, slots);
+        return;
+    }
     if (t.op >= 4) {
-        // ops 4-8: one element per thread per trip, fp32 partials per thread, fp64 across threads
+        // ops 4-9: one element per thread per trip, fp32 partials per thread, fp64 across threads
         const bool masked = t.op >= 6;
         const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;
         float accl = 0.f;
@@ -194,8 +256,9 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
 }
 
 // ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * ([sign*a - 1 < 0] + [sign*a - 1 == 0] / 2);  op 1: 1;
-// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-8: term_df.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
-// gives each side half the gradient.  The masked ops' denominators are folded into gslot by the caller.
+// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10: term_df.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
+// gives each side half the gradient.  The masked ops' denominators are folded into gslot by the caller.  With t.add the
+// result is added to add_i (which may be ga itself: each element is read before the same thread writes it).
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
     const LossTerm t = terms[blockIdx.y];
     if (!t.ga) return;
@@ -205,7 +268,8 @@ __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __
         const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;
         for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
             const float l = masked ? term_label(t, i, sh, sw) : 0.f;
-            t.ga[i] = g * term_df(t, __ldg(t.a + i), i, l);
+            const float v = g * term_df(t, __ldg(t.a + i), i, l);
+            t.ga[i] = t.add ? t.add[i] + v : v;
         }
         return;
     }
@@ -219,7 +283,8 @@ __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __
         else if (t.op == 1) d = 1.f;
         else if (t.op == 2) { const float df = a - __ldg(t.b + i); d = df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f); }
         else d = 2.f * (a - __ldg(t.b + i));
-        t.ga[i] = g * d;
+        const float v = g * d;
+        t.ga[i] = t.add ? t.add[i] + v : v;
     }
 }
 

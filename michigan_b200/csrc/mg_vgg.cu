@@ -348,12 +348,23 @@ __global__ void __launch_bounds__(256) hair_avg_lab_bwd_kernel(const float* __re
 // calc_mean_std (loss.py:624-632) from the fp64 per-(n, c) sums of mg_in_stats ([N][2][C]: sum x, then sum x^2, over M pixels):
 //   mu = S1 / M,  var = (S2 - S1 mu) / (M - 1) (unbiased; clamped at 0 against cancellation),  sigma = sqrt(var + 1e-5).
 // calc_style_loss (loss.py:668-683, remove_background False) of one tap: MSE(mu_f, mu_t) + MSE(sigma_f, sigma_t) over N x C.
+//
+// Masked mode (cnt_f, cnt_t set; calc_mean_std_mask, loss.py:634-654, and calc_style_loss with remove_background, 679-694): the
+// sums are mg_loss_reduce op 10's (sum m x, sum m x^2 per (n, c)) and cnt the per-image sum m, m binary (m^2 = m), D = cnt:
+//   mu = S1 / (D + eps),  var = sum m (x - mu)^2 / (D + eps) + eps = (S2 - mu (2 S1 - mu D)) / (D + eps) + eps  (biased, eps
+//   twice, no M - 1: no pixel-count refusal; an image without mask pixels gives mu = 0, sigma = sqrt(eps)).
+// coef then holds op 10's backward table: mu' = mu (1 + eps / (D + eps)), A = 2 (mu_f - mu_t) / (N C (D + eps)),
+// B = 2 (sigma_f - sigma_t) / (N C sigma_f (D + eps)).  mu' folds in the term -(m_p / (D + eps)) sum_q m_q (x_q - mu) =
+// -m_p mu eps / (D + eps) of d var / d x_p, which is not zero because of the eps in mu's denominator.
 struct StyleTap {
     const double* sums_f;   // [N][2][C] of the fake images
     const double* sums_t;   // [N][2][C] of the style targets
-    float* coef;            // [N][3][C] out: mu_f, mu_f - mu_t, (sigma_f - sigma_t) / sigma_f
+    float* coef;            // [N][3][C] out: mu_f, mu_f - mu_t, (sigma_f - sigma_t) / sigma_f  (masked: mu', A, B)
     long long M;
     int N, C;
+    // appended: the masked mode (both null: unmasked)
+    const double* cnt_f;    // [N] sum m of the fake images' masks
+    const double* cnt_t;    // [N] sum m of the style targets' masks
 };
 constexpr int kMaxStyleTaps = 8;
 struct StyleTaps {
@@ -376,12 +387,24 @@ __global__ void __launch_bounds__(512) style_loss_fwd_kernel(const StyleTaps tap
             const int n = i / t.C, c = i - n * t.C;
             const double* f = t.sums_f + (size_t)n * 2 * t.C;
             const double* r = t.sums_t + (size_t)n * 2 * t.C;
+            float* co = t.coef + (size_t)n * 3 * t.C + c;
+            if (t.cnt_f) {
+                const double Df = t.cnt_f[n], Dt = t.cnt_t[n], ef = Df + kStyleEps, et = Dt + kStyleEps;
+                const double mf = f[c] / ef, mt = r[c] / et;
+                const double sf = sqrt(fmax(f[t.C + c] - mf * (2.0 * f[c] - mf * Df), 0.0) / ef + kStyleEps);
+                const double st = sqrt(fmax(r[t.C + c] - mt * (2.0 * r[c] - mt * Dt), 0.0) / et + kStyleEps);
+                const double dm = mf - mt, ds = sf - st;
+                s += dm * dm + ds * ds;
+                co[0] = (float)(mf * (1.0 + kStyleEps / ef));
+                co[t.C] = (float)(2.0 * dm / ((double)NC * ef));
+                co[2 * t.C] = (float)(2.0 * ds / ((double)NC * sf * ef));
+                continue;
+            }
             const double mf = f[c] / M, mt = r[c] / M;
             const double sf = sqrt(fmax((f[t.C + c] - f[c] * mf) / (M - 1.0), 0.0) + kStyleEps);
             const double st = sqrt(fmax((r[t.C + c] - r[c] * mt) / (M - 1.0), 0.0) + kStyleEps);
             const double dm = mf - mt, ds = sf - st;
             s += dm * dm + ds * ds;
-            float* co = t.coef + (size_t)n * 3 * t.C + c;
             co[0] = (float)mf;
             co[t.C] = (float)dm;
             co[2 * t.C] = (float)(ds / sf);
@@ -606,7 +629,8 @@ extern "C" int mg_style_loss_fwd(const void* taps_host, int n_taps, double* loss
         const StyleTap& t = static_cast<const StyleTap*>(taps_host)[k];
         if (!t.sums_f || !t.sums_t || !t.coef) return set_error(-1, "mg_style_loss_fwd: null pointer in tap %d", k);
         if (t.N < 1 || t.C < 4 || t.C % 4 != 0) return set_error(-2, "mg_style_loss_fwd: bad size in tap %d", k);
-        if (t.M < 2)
+        if ((!t.cnt_f) != (!t.cnt_t)) return set_error(-1, "mg_style_loss_fwd: tap %d has one mask count but not the other", k);
+        if (!t.cnt_f && t.M < 2)
             return set_error(-2, "mg_style_loss_fwd: tap %d has %lld pixel(s); the unbiased variance needs at least 2 (crop size >= 32)", k,
                              t.M);
         if (!aligned16(t.coef)) return set_error(-4, "mg_style_loss_fwd: coefficient table of tap %d must be 16-byte aligned", k);

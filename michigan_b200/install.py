@@ -83,6 +83,8 @@ def _patch_runtime():
 
       * `util.save_network` (util/util.py:195-200) -> michigan_b200.checkpoint.save_network: rank 0 only, atomic rename,
         barrier, no round trip of the whole network through the CPU;
+      * `Pix2PixModel.__init__`: under --remove_background it sets opt.mask_vgg_losses, so the installed VGGLoss and
+        StyleContentLoss compute the reference's hair-masked terms (networks.loss.masked_vgg_losses);
       * `Pix2PixModel.compute_generator_loss` (pix2pix_model.py:257-365): the discriminators' parameters (netD, and netD2
         of --unpairTrain, which judges the generator in the unpaired stage, pix2pix_model.py:568-572) do not require grad
         while the GENERATOR's loss is back-propagated - the reference computes those gradients and throws them away
@@ -110,4 +112,14 @@ def _patch_runtime():
                     p.requires_grad_(r)
 
         cls.compute_generator_loss = compute_generator_loss
+        orig_init = cls.__init__
+
+        def __init__(self, opt, *a, **k):
+            # the reference's --remove_background masks its VGG, content and style losses too (loss.py:187-207, 634-711): opt
+            # into the masked terms of networks.loss.VGGLoss / StyleContentLoss, which refuse the flag alone
+            if getattr(opt, "remove_background", False):
+                opt.mask_vgg_losses = True
+            orig_init(self, opt, *a, **k)
+
+        cls.__init__ = __init__
         cls._mg_patched = True

@@ -24,14 +24,18 @@ class _Term(C.Structure):
                 # appended for ops 4-8 (zero for ops 0-3)
                 ("target", C.c_float), ("den_slot", C.c_int32), ("label", C.c_void_p), ("label_ns", C.c_longlong),
                 ("C", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
-                ("channels_last", C.c_int32)]
+                ("channels_last", C.c_int32),
+                # appended for the accumulating backward (null: ga is written, not accumulated)
+                ("add", C.c_void_p)]
 
 
 OP_HINGE_D, OP_SUM, OP_L1, OP_SQ = 0, 1, 2, 3
 # gan_mode 'original' / 'ls' against a constant target; the --remove_background terms, masked by the resized hair label
 OP_BCE, OP_SQ_T, OP_WSUM, OP_HINGE_MASK, OP_L1_MASK = 4, 5, 6, 7, 8
-MASKED_OPS = (OP_WSUM, OP_HINGE_MASK, OP_L1_MASK)
-DEN_EPS = 1e-5          # loss.py:111, 114, 117, 160: sum(label1) * c + 1e-5
+# --remove_background in VGGLoss / StyleContentLoss: the masked content term and the masked channel moments of one VGG tap
+OP_SQ_MASK, OP_MOMENTS = 9, 10
+MASKED_OPS = (OP_WSUM, OP_HINGE_MASK, OP_L1_MASK, OP_SQ_MASK)      # one scalar term over its own sum(label1) * c + 1e-5
+DEN_EPS = 1e-5          # loss.py:111, 114, 117, 160, 196, 677: sum(label1) * c + 1e-5
 _table_cache = {}
 
 
@@ -79,10 +83,24 @@ def _device_table(terms, device):
     return buf
 
 
-def _term(s, a, b, ga, out_slot, den_slot):
+def _fold_masked(nums, dens):
+    """The masked terms' values sum_k nums[k] / (dens[k] + 1e-5), formed on the device (no host synchronisation), and the
+    1 / (dens + 1e-5) that scale their gradients (_masked_gslots)."""
+    inv = 1.0 / (dens + DEN_EPS)
+    return (nums * inv).sum(), inv
+
+
+def _masked_gslots(g, inv):
+    """The gradient slots of masked terms: the upstream gradient g over each term's denominator, fp32."""
+    return (g.double() * inv).float()
+
+
+def _term(s, a, b, ga, out_slot, den_slot, add=None):
+    """The _Term record of spec s on a ([N,C,h,w], NCHW or channels-last for the masked ops); ga, add: gradient pointers."""
     t = _Term(a.data_ptr(), b.data_ptr() if b is not None else None, ga, a.numel(), float(s.scale), float(s.sign), s.op, out_slot)
     t.target = float(s.target)
-    if s.op in MASKED_OPS:
+    t.add = add
+    if s.op in MASKED_OPS or s.op == OP_MOMENTS:
         lab = s.label
         t.den_slot, t.label, t.label_ns = den_slot, lab.data_ptr(), lab.stride(0)
         t.C, t.h, t.w = a.shape[1], a.shape[2], a.shape[3]
@@ -132,9 +150,9 @@ class _LossFn(torch.autograd.Function):
         if not m:
             return slots.float()
         # loss.py:111, 114, 117, 160: each masked term divided by its own sum(label1) * c + 1e-5, on the device
-        ctx.inv = 1.0 / (slots[nslots + m:] + DEN_EPS)
+        val, ctx.inv = _fold_masked(slots[nslots:nslots + m], slots[nslots + m:])
         out = slots[:nslots].clone()
-        out[spec[masked[0]].slot] += (slots[nslots:nslots + m] * ctx.inv).sum()
+        out[spec[masked[0]].slot] += val
         return out.float()
 
     @staticmethod
@@ -160,7 +178,7 @@ class _LossFn(torch.autograd.Function):
         if ctx.inv is not None:
             m = ctx.inv.numel()
             slot = next(s.slot for s in ctx.spec if s.op in MASKED_OPS)
-            g = torch.cat([g, (g[slot].double() * ctx.inv).float(), torch.zeros(m, device=dev, dtype=torch.float32)])
+            g = torch.cat([g, _masked_gslots(g[slot], ctx.inv), torch.zeros(m, device=dev, dtype=torch.float32)])
         _lib.check(_lib.load().mg_loss_reduce_bwd(table.data_ptr(), len(terms), g.data_ptr(), ops._stream()), "mg_loss_reduce_bwd")
         grads = []
         for i, (shape, stride, dstride) in enumerate(ctx.shapes):
@@ -319,7 +337,8 @@ VGG_WEIGHTS = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
 
 
 def style_min_size_error(h, w):
-    """The style loss's unbiased variance needs at least 2 pixels at relu5_1 (h/16 x w/16); the reference returns NaN below."""
+    """The style loss's unbiased variance needs at least 2 pixels at relu5_1 (h/16 x w/16); the reference returns NaN below.
+    The masked style loss of --remove_background has no such limit (its variance is biased)."""
     if (h // 16) * (w // 16) < 2:
         return NotImplementedError("michigan_b200: the style loss needs at least 2 pixels at relu5_1 (crop_size >= 32), got %dx%d"
                                    % (h, w))
@@ -336,10 +355,12 @@ class _VGGObjectiveFn(torch.autograd.Function):
 
     want = (l1, content, style); a term not asked for returns None.  style_img None: the style targets are the tag half (2N
     batch).  Backward: mg_loss_reduce_bwd writes the L1 tap gradients, mg_style_tap_grad adds the style gradient (and at relu5_1
-    the content gradient) in place, then the hand-written VGG19 backward takes them down to d fake."""
+    the content gradient) in place, then the hand-written VGG19 backward takes them down to d fake.
+
+    labels = (tag label, style label), [N,1,H,W] hair labels (_hair_label): --remove_background, _MaskedVGGTerms."""
 
     @staticmethod
-    def forward(ctx, vgg, weights, want, fake, tag, style_img):
+    def forward(ctx, vgg, weights, want, fake, tag, style_img, labels=None):
         l1, content, style = want
         n = fake.shape[0]
         parts = [fake.detach(), tag.detach()] + ([style_img.detach()] if style and style_img is not None else [])
@@ -347,6 +368,11 @@ class _VGGObjectiveFn(torch.autograd.Function):
         taps, S = vgg.run(x8, n_save=n if ctx.needs_input_grad[3] else 0)
         del x8
         pairs = [(t[:n], t[n:2 * n]) for t in taps]
+        ctx.masked = None
+        if labels is not None:
+            ctx.masked = _MaskedVGGTerms(taps, n, n if style_img is None else 2 * n, weights, want, labels)
+            ctx.vgg, ctx.want, ctx.pairs, ctx.S, ctx.hw = vgg, want, pairs, S, tuple(fake.shape[2:])
+            return ctx.masked.outputs
         out_l1 = out_c = out_s = None
         if l1 or content:
             terms = [_Term(a.data_ptr(), b.data_ptr(), None, a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
@@ -377,6 +403,12 @@ class _VGGObjectiveFn(torch.autograd.Function):
         pairs = ctx.pairs
         dev = pairs[0][0].device
         grads = [None] * len(pairs)
+        if ctx.masked is not None:
+            grads = ctx.masked.backward(pairs, g_l1, g_c, g_s)
+            ctx.pairs = ctx.masked = None
+            dimg = ctx.vgg.backward(ctx.S, grads, ctx.hw)
+            ctx.S = None
+            return None, None, None, dimg, None, None, None
         if l1:
             grads = [torch.empty_like(a) for a, _ in pairs]
             terms = [_Term(a.data_ptr(), b.data_ptr(), ga.data_ptr(), a.numel(), float(w / a.numel()), 1.0, OP_L1, 0)
@@ -396,21 +428,137 @@ class _VGGObjectiveFn(torch.autograd.Function):
         ctx.pairs = ctx.coefs = None
         dimg = ctx.vgg.backward(ctx.S, grads, ctx.hw)
         ctx.S = None
-        return None, None, None, dimg, None, None
+        return None, None, None, dimg, None, None, None
+
+
+def _nchw(t):
+    """The [N,C,h,w] channels-last view of an NHWC VGG tap (what the masked ops' records describe)."""
+    return t.permute(0, 3, 1, 2)
+
+
+class _MaskedVGGTerms:
+    """The --remove_background VGG terms of one _VGGObjectiveFn call (loss.py:187-207, 634-711), l the tag label and ls the
+    style label resized (nearest) to each tap:
+
+      l1       VGGLoss.L1_loss_mask: sum_i w_i sum |x_i l - y_i l| / (sum l c + 1e-5)      op 8, one term per tap
+      content  calc_content_loss: sum (x_5 l - t_5 l)^2 / (sum l c + 1e-5)                 op 9 at relu5_1
+      style    calc_style_loss with calc_mean_std_mask: the fake taps' moments under ls, the style targets' under l  op 10, two
+               terms per tap (the reference crosses the masks: calc_style_loss(fake, style, style_label, content_label) masks
+               the fake features with the style image's hair and the style features with the tag's), then mg_style_loss_fwd
+               in its masked mode
+
+    Forward: ONE mg_loss_reduce launch for every term above (one fp64 slot buffer; the denominators folded on the device by
+    _fold_masked) and one mg_style_loss_fwd.  Backward: op 8 writes the L1 tap gradients, op 10 adds the style gradients, op 9
+    adds the content gradient at relu5_1: three mg_loss_reduce_bwd launches, as no two terms of one launch may write one tensor."""
+
+    def __init__(self, taps, n, t0, weights, want, labels):
+        l1, content, style = want
+        lab_tag, lab_style = labels
+        dev = taps[0].device
+        self.want, self.weights, self.labels = want, weights, labels
+        specs = []                                          # (spec, a, b, out_slot, den_slot)
+        off = 0
+        if l1:
+            self.l1_off = off
+            k = len(taps)
+            for i, (t, w) in enumerate(zip(taps, weights)):
+                specs.append((_Spec(OP_L1_MASK, 0, None, float(w), 1.0, 0, label=lab_tag), t[:n], t[n:2 * n], off + i, off + k + i))
+            off += 2 * k
+        if content:
+            self.c_off = off
+            t = taps[-1]
+            specs.append((_Spec(OP_SQ_MASK, 0, None, 1.0, 1.0, 0, label=lab_tag), t[:n], t[n:2 * n], off, off + 1))
+            off += 2
+        moments = []
+        if style:
+            for t in taps:
+                c = t.shape[3]
+                for half, lab in ((t[:n], lab_style), (t[t0:t0 + n], lab_tag)):
+                    specs.append((_Spec(OP_MOMENTS, 0, None, 1.0, 1.0, 0, label=lab), half, None, off, off + 2 * n * c))
+                    moments.append((off, c))
+                    off += 2 * n * c + n
+        slots = torch.zeros(off, device=dev, dtype=torch.float64)
+        terms = [_term(sp, _nchw(a), b, None, o, d) for sp, a, b, o, d in specs]
+        _lib.check(_lib.load().mg_loss_reduce(_device_table(terms, dev).data_ptr(), len(terms), slots.data_ptr(), ops._stream()),
+                   "mg_loss_reduce")
+        out_l1 = out_c = out_s = None
+        if l1:
+            k = len(taps)
+            val, self.inv_l1 = _fold_masked(slots[self.l1_off:self.l1_off + k], slots[self.l1_off + k:self.l1_off + 2 * k])
+            out_l1 = val.float()
+        if content:
+            val, self.inv_c = _fold_masked(slots[self.c_off:self.c_off + 1], slots[self.c_off + 1:self.c_off + 2])
+            out_c = val.float()
+        self.coefs = None
+        if style:
+            recs = []
+            for t, (fo, c), (to, _) in zip(taps, moments[0::2], moments[1::2]):
+                recs.append((slots[fo:fo + 2 * n * c].view(n, 2, c), slots[to:to + 2 * n * c].view(n, 2, c), t.shape[1] * t.shape[2],
+                             slots[fo + 2 * n * c:fo + 2 * n * c + n], slots[to + 2 * n * c:to + 2 * n * c + n]))
+            loss, self.coefs = ops.style_loss_fwd(recs)
+            out_s = loss.float().reshape(())
+        self.outputs = (out_l1, out_c, out_s)
+
+    def backward(self, pairs, g_l1, g_c, g_s):
+        l1, content, style = self.want
+        lab_tag, lab_style = self.labels
+        dev = pairs[0][0].device
+        lib = _lib.load()
+        grads = [None] * len(pairs)
+        if l1:
+            grads = [torch.empty_like(a) for a, _ in pairs]
+            gs = _masked_gslots(g_l1.reshape(()), self.inv_l1).contiguous()
+            terms = [_term(_Spec(OP_L1_MASK, 0, None, float(w), 1.0, 0, label=lab_tag), _nchw(a), b, ga.data_ptr(), i, 0)
+                     for i, ((a, b), ga, w) in enumerate(zip(pairs, grads, self.weights))]
+            _lib.check(lib.mg_loss_reduce_bwd(_device_table(terms, dev).data_ptr(), len(terms), gs.data_ptr(), ops._stream()),
+                       "mg_loss_reduce_bwd")
+        if style:
+            gs = g_s.reshape(1).contiguous().float()
+            terms = []
+            for i, (a, _) in enumerate(pairs):
+                add = grads[i].data_ptr() if grads[i] is not None else None
+                if grads[i] is None:
+                    grads[i] = torch.empty_like(a)
+                terms.append(_term(_Spec(OP_MOMENTS, 0, None, 1.0, 1.0, 0, label=lab_style), _nchw(a), self.coefs[i],
+                                   grads[i].data_ptr(), 0, 0, add=add))
+            _lib.check(lib.mg_loss_reduce_bwd(_device_table(terms, dev).data_ptr(), len(terms), gs.data_ptr(), ops._stream()),
+                       "mg_loss_reduce_bwd")
+        if content:
+            a, b = pairs[-1]
+            gs = _masked_gslots(g_c.reshape(()), self.inv_c).contiguous()
+            add = grads[-1].data_ptr() if grads[-1] is not None else None
+            if grads[-1] is None:
+                grads[-1] = torch.empty_like(a)
+            terms = [_term(_Spec(OP_SQ_MASK, 0, None, 1.0, 1.0, 0, label=lab_tag), _nchw(a), b, grads[-1].data_ptr(), 0, 0, add=add)]
+            _lib.check(lib.mg_loss_reduce_bwd(_device_table(terms, dev).data_ptr(), 1, gs.data_ptr(), ops._stream()),
+                       "mg_loss_reduce_bwd")
+        self.coefs = None
+        return grads
 
 
 def _same_image(a, b):
     return a is b or (a.shape == b.shape and bool(torch.equal(a, b)))
 
 
-def vgg_objective(vgg, fake, tag, style_image=None, l1=False, content=False, style=False, weights=VGG_WEIGHTS):
+def vgg_objective(vgg, fake, tag, style_image=None, l1=False, content=False, style=False, weights=VGG_WEIGHTS, label=None,
+                  style_label=None):
     """(l1, content, style) of fake against tag (and the style image) from one VGG19 pass (_VGGObjectiveFn); None for a term not
     asked for.  A style image equal to the tag (paired training loads the same file for both) is not run through VGG19 again:
-    the style targets then come from the tag half."""
-    if style:
+    the style targets then come from the tag half.
+
+    label (the tag's [N,1,H,W] hair label) selects --remove_background: every term is masked by it, except that the fake's
+    style statistics are masked by style_label (the style image's hair label), as the reference does."""
+    masked = label is not None
+    labels = None
+    if masked:
+        if style and style_label is None:
+            raise ValueError("--remove_background: the style loss needs the style image's hair label")
+        labels = (_hair_label(label, fake), _hair_label(style_label, fake) if style else None)
+    if style and not masked:
         err = style_min_size_error(*fake.shape[2:])
         if err is not None:
             raise err
+    if style:
         if style_image is None or _same_image(style_image, tag):
             style_image = None
         else:
@@ -422,37 +570,61 @@ def vgg_objective(vgg, fake, tag, style_image=None, l1=False, content=False, sty
     dev = fake.device
     if next(vgg.parameters()).device != dev:
         vgg.to(dev)
-    return _VGGObjectiveFn.apply(vgg, weights, (bool(l1), bool(content), bool(style)), fake, tag.float(), style_image)
+    return _VGGObjectiveFn.apply(vgg, weights, (bool(l1), bool(content), bool(style)), fake, tag.float(), style_image, labels)
+
+
+def masked_vgg_losses(opt, who):
+    """Whether the VGG, content and style losses run hair-masked: opt.remove_background together with opt.mask_vgg_losses.
+    --remove_background alone is refused here with NotImplementedError, as before the masked terms existed, so that a
+    configuration that used to be rejected does not start training a different objective unannounced; mask_vgg_losses opts
+    into the reference's masked terms (install() sets it for the reference's own Pix2PixModel, whose --remove_background
+    always meant them)."""
+    if not getattr(opt, "remove_background", False):
+        return False
+    if not getattr(opt, "mask_vgg_losses", False):
+        raise NotImplementedError("michigan_b200: %s with --remove_background computes the hair-masked terms only when "
+                                  "opt.mask_vgg_losses is set (install() sets it for the reference's model)" % who)
+    return True
 
 
 class VGGLoss(nn.Module):
-    """loss.py:178-207 (remove_background=False): sum_i w_i * L1(vgg(x)_i, vgg(y)_i.detach()), w = 1/32, 1/16, 1/8, 1/4, 1.
-    The image is fed to VGG19 in [-1, 1] without ImageNet normalisation, as the reference does.  The weights are never
-    downloaded (VGG19: `state_dict` or torchvision's cache file)."""
+    """loss.py:178-207: sum_i w_i * L1(vgg(x)_i, vgg(y)_i.detach()), w = 1/32, 1/16, 1/8, 1/4, 1; under --remove_background
+    (with opt.mask_vgg_losses, masked_vgg_losses) the hair-masked L1_loss_mask of each tap, sum |x_i l - y_i l| / (sum l * c
+    + 1e-5), l = label resized (nearest) to the tap.  The image is fed to VGG19 in [-1, 1] without ImageNet normalisation, as
+    the reference does.  The weights are never downloaded (VGG19: `state_dict` or torchvision's cache file)."""
 
     def __init__(self, opt=None, state_dict=None):
         super().__init__()
-        if getattr(opt, "remove_background", False):
-            raise NotImplementedError("michigan_b200: --remove_background is not implemented")
+        self.masked = masked_vgg_losses(opt, "VGGLoss")
         from .architecture import VGG19
         self.vgg = VGG19(state_dict=state_dict)
         self.weights = list(VGG_WEIGHTS)
         self.opt = opt
 
     def forward(self, x, y, label=None):
+        if self.masked:
+            return vgg_objective(self.vgg, x, y, l1=True, weights=self.weights, label=_required(label, "VGGLoss"))[0]
         return vgg_objective(self.vgg, x, y, l1=True, weights=self.weights)[0]
 
 
+def _required(label, who):
+    if label is None:
+        raise ValueError("%s: --remove_background needs the hair label" % who)
+    return label
+
+
 class StyleContentLoss(nn.Module):
-    """loss.py:656-711 (remove_background=False): (loss_c, loss_s) = forward(fake_image, style_image, content_image), with
+    """loss.py:656-711: (loss_c, loss_s) = forward(fake_image, style_image, content_image, style_label, content_label), with
     loss_c = MSE(relu5_1(fake), relu5_1(content).detach()) and loss_s = sum over the five taps of MSE(mu_fake, mu_style) +
-    MSE(sigma_fake, sigma_style) (calc_mean_std: per (n, c), unbiased variance + 1e-5).  One VGG19 pass over fake || content
-    (|| style, unless it equals content) and one backward (_VGGObjectiveFn).  `vgg` shares another loss's VGG19 instance."""
+    MSE(sigma_fake, sigma_style) (calc_mean_std: per (n, c), unbiased variance + 1e-5).  Under --remove_background (with
+    opt.mask_vgg_losses, masked_vgg_losses) the content
+    term is masked by content_label over sum(label) * c + 1e-5, and the statistics are calc_mean_std_mask's (biased variance,
+    the fake masked by style_label, the style image by content_label: the reference's crossing).  One VGG19 pass over fake ||
+    content (|| style, unless it equals content) and one backward (_VGGObjectiveFn).  `vgg` shares another loss's VGG19."""
 
     def __init__(self, opt=None, vgg=None, state_dict=None):
         super().__init__()
-        if getattr(opt, "remove_background", False):
-            raise NotImplementedError("michigan_b200: --remove_background is not implemented (calc_mean_std_mask / masked content loss)")
+        self.masked = masked_vgg_losses(opt, "StyleContentLoss")
         if vgg is None:
             from .architecture import VGG19
             vgg = VGG19(state_dict=state_dict)
@@ -460,7 +632,12 @@ class StyleContentLoss(nn.Module):
         self.opt = opt
 
     def forward(self, fake_image, style_image, content_image, style_label=None, content_label=None):
-        _, loss_c, loss_s = vgg_objective(self.vgg, fake_image, content_image, style_image, content=True, style=True)
+        if self.masked:
+            _, loss_c, loss_s = vgg_objective(self.vgg, fake_image, content_image, style_image, content=True, style=True,
+                                              label=_required(content_label, "StyleContentLoss"),
+                                              style_label=_required(style_label, "StyleContentLoss"))
+        else:
+            _, loss_c, loss_s = vgg_objective(self.vgg, fake_image, content_image, style_image, content=True, style=True)
         return loss_c, loss_s
 
 

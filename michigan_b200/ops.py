@@ -707,9 +707,9 @@ def hair_avg_lab_bwd(fake, mask_fake, sums, g):
 
 
 class StyleTap(C.Structure):
-    """One record of mg_style_loss_fwd's host table (include/michigan_b200.h)."""
+    """One record of mg_style_loss_fwd's host table (include/michigan_b200.h); cnt_f / cnt_t set select the masked mode."""
     _fields_ = [("sums_f", C.c_void_p), ("sums_t", C.c_void_p), ("coef", C.c_void_p), ("M", C.c_longlong), ("N", C.c_int32),
-                ("C", C.c_int32)]
+                ("C", C.c_int32), ("cnt_f", C.c_void_p), ("cnt_t", C.c_void_p)]
 
 
 def channel_sums(x):
@@ -723,15 +723,21 @@ def channel_sums(x):
 
 def style_loss_fwd(taps):
     """taps: list of (sums_fake [N,2,C], sums_target [N,2,C], M) -> ([1] float64 loss sum over the taps, [coef [N,3,C] per tap]).
+    A tap (sums_fake, sums_target, M, cnt_fake [N], cnt_target [N]) takes the masked mode: the sums and the per-image mask
+    counts of mg_loss_reduce op 10, the reference's calc_mean_std_mask, and coef is op 10's backward table.
     One mg_style_loss_fwd launch for every tap."""
     recs, coefs = [], []
-    for sf, st, M in taps:
+    for tap in taps:
+        sf, st, M = tap[:3]
+        cf, ct = tap[3:] if len(tap) > 3 else (None, None)
         _chk(sf, "sums_f", torch.float64); _chk(st, "sums_t", torch.float64)
+        _chk(cf, "cnt_f", torch.float64); _chk(ct, "cnt_t", torch.float64)
         N, _, Cc = sf.shape
         assert st.shape == sf.shape, (st.shape, sf.shape)
+        assert cf is None or (cf.numel() == N and ct.numel() == N), (cf, ct)
         coef = torch.empty((N, 3, Cc), device=sf.device, dtype=torch.float32)
         coefs.append(coef)
-        recs.append(StyleTap(_p(sf), _p(st), _p(coef), int(M), N, Cc))
+        recs.append(StyleTap(_p(sf), _p(st), _p(coef), int(M), N, Cc, _p(cf), _p(ct)))
     loss = torch.zeros(1, device=taps[0][0].device, dtype=torch.float64)
     table = (StyleTap * len(recs))(*recs)
     check(_lib.load().mg_style_loss_fwd(C.cast(table, C.c_void_p), len(recs), _p(loss), _stream()), "mg_style_loss_fwd")

@@ -19,6 +19,9 @@ def make_opt(is_train=True, **overrides):
         no_orientation=False, add_feat_zeros=False, add_th=64, clip_th=300, use_clip=False, orient_random_disturb=False,
         expand_mask_be=True, expand_th=5, semantic_nc=2, inpaint_mode="ref", only_blend=False, unpairTrain=False,
         curr_step=1, remove_background=False,
+        # not a reference option: with remove_background, also mask the VGG, content and style losses (networks.loss.
+        # masked_vgg_losses; install() sets it on the reference's own options)
+        mask_vgg_losses=False,
         # train options
         ndf=64, netD="multiscale", netD_subarch="n_layer", num_D=2, n_layers_D=4, lambda_feat=1.0, no_gan_loss=False,
         no_ganFeat_loss=False, gan_mode="hinge", no_TTUR=False, lr=0.0002, beta1=0.5, beta2=0.999, wide_edge=2.0,

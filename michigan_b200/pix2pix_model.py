@@ -33,7 +33,8 @@ class Pix2PixModel(torch.nn.Module):
                 raise NotImplementedError("michigan_b200: --%s is outside the hot path (SURVEY.md §8)" % flag)
         # Every term of the reference's generator objective for curr_step 1 (pix2pix_model.py:296-345) is computed here: GAN
         # (any --gan_mode), GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT, CONFIDENCE, each dropped by its --no_*
-        # flag.  GANLoss and GANFeatLoss take --remove_background; VGGLoss and StyleContentLoss refuse it, and LabColorLoss
+        # flag.  GANLoss and GANFeatLoss take --remove_background; VGGLoss and StyleContentLoss take it together with
+        # mask_vgg_losses (the reference's hair-masked terms, networks.loss.masked_vgg_losses) and refuse it alone; LabColorLoss
         # refuses --balance_Lab.
         self.netIG = None
         if getattr(opt, "use_ig", False):
@@ -201,7 +202,7 @@ class Pix2PixModel(torch.nn.Module):
         # pix2pix_model.py:300-340, in the reference's key order (GAN, GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT,
         # CONFIDENCE): VGG, background, rgb and lab only when ref is tag, content and style whenever curr_step is 1
         if self.opt.curr_step == 1:
-            vgg, content, style = self._vgg_terms(fake_image, image_ref, image_tag, ref_is_tag)
+            vgg, content, style = self._vgg_terms(fake_image, image_ref, image_tag, ref_is_tag, label_tag, input_ref[:, 1:2])
             if vgg is not None:
                 G_losses["VGG"] = vgg * self.opt.lambda_vgg
             if content is not None:
@@ -222,17 +223,21 @@ class Pix2PixModel(torch.nn.Module):
                 G_losses["CONFIDENCE"] = confidence_loss * self.opt.lambda_confidence
         return G_losses, fake_image
 
-    def _vgg_terms(self, fake_image, image_ref, image_tag, ref_is_tag):
+    def _vgg_terms(self, fake_image, image_ref, image_tag, ref_is_tag, label_tag, label_ref):
         """(VGG, content, style), None for a term that is off: one VGG19 pass over fake || tag (|| ref, unless it equals tag) for
-        all of them (networks.loss.vgg_objective); VGG alone goes through criterionVGG, as before."""
+        all of them (networks.loss.vgg_objective); VGG alone goes through criterionVGG, as before.  Under --remove_background
+        the terms are masked by the tag's hair label, and the fake's style statistics by the reference's (pix2pix_model.py:
+        303-315: label_tag, style_label = input_ref[:, 1], content_label = input_tag[:, 1])."""
         l1 = not getattr(self.opt, "no_vgg_loss", False) and ref_is_tag
         content = not getattr(self.opt, "no_content_loss", False)
         style = not getattr(self.opt, "no_style_loss", False)
+        masked = self.criterionStyleContent.masked if (content or style) else False
         if not (content or style):
-            return (self.criterionVGG(fake_image, image_tag) if l1 else None), None, None
+            return (self.criterionVGG(fake_image, image_tag, label_tag) if l1 else None), None, None
         crit = self.criterionStyleContent
         return vgg_objective(crit.vgg, fake_image, image_tag, image_ref, l1=l1, content=content, style=style,
-                             weights=self.criterionVGG.weights if l1 else None)
+                             weights=self.criterionVGG.weights if l1 else None, label=label_tag if masked else None,
+                             style_label=label_ref if masked else None)
 
     def compute_discriminator_loss(self, input_ref, input_tag, image_ref, image_tag, orient_mask, noise):
         with torch.no_grad():

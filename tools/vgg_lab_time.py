@@ -5,7 +5,11 @@ eagerly on CUDA (cuDNN) with the same seeded weights.  The VGG terms of the defa
 (VGG L1 + content + style, ref == tag and ref != tag) and as VGGLoss + StyleContentLoss called separately (what the reference's
 Pix2PixModel does under install()), with the style statistics and tap-gradient kernels on their own.
 
-    python tools/vgg_lab_time.py OUT_DIR [--batch 8] [--steps 5] [--rounds 3]
+    python tools/vgg_lab_time.py OUT_DIR [--batch 8] [--steps 5] [--rounds 3] [--remove_background]
+
+--remove_background times only the hair-masked VGG terms: the combined VGG L1 + content + style pass (_VGGObjectiveFn, ref !=
+tag, the tag and reference labels of the synthetic batch) and the default-objective train step, each masked against unmasked,
+alternated in one process (OUT_DIR/vgg_lab_time_remove_background.json).
 
 Batch 8, 512x512, synthetic inputs.  Writes OUT_DIR/vgg_lab_time.json and prints one line per measurement, headed by the GPU's
 name, power limit and maximum SM clock (read-only nvidia-smi query).  Algorithmic rates: VGG = fake forward + real forward +
@@ -68,9 +72,12 @@ def main():
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--remove_background", action="store_true")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("vgg_lab_time.py needs a CUDA device")
+    if a.remove_background:
+        return remove_background_times(a)
     import oracle_vgg_lab as ovl
     from kernel_times import DEFAULT_LOSSES, README_LOSSES, build_model
     from michigan_b200 import ops
@@ -176,6 +183,57 @@ def main():
     print("Lab loss fwd+bwd: %.3f ms, %.0f GB/s algorithmic" % (ms_l, nbytes / ms_l / 1e6))
     os.makedirs(a.out_dir, exist_ok=True)
     with open(os.path.join(a.out_dir, "vgg_lab_time.json"), "w") as f:
+        json.dump(res, f, indent=1)
+
+
+def remove_background_times(a):
+    """The masked VGG terms and the default-objective train step against the unmasked ones, alternated."""
+    from kernel_times import DEFAULT_LOSSES, build_model
+    from michigan_b200.networks import VGGLoss
+    from michigan_b200.networks.loss import vgg_objective
+    from michigan_b200.networks.sync_batchnorm import DataParallelWithCallback
+    from michigan_b200.options import make_opt
+    from michigan_b200.pix2pix_model import train_iteration
+    from michigan_b200.synth import synthetic_batch, vgg19_state_dict
+
+    info = gpu_info()
+    print("GPU:", info)
+    n = a.batch
+    data = synthetic_batch(n, SIZE, 1234)
+    dev = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in data.items()}
+    res = {"gpu": info, "batch": n, "size": SIZE}
+    legs = {}
+    for name, rb in (("default", False), ("default_remove_background", True)):
+        model = build_model(n, remove_background=rb, mask_vgg_losses=rb, **DEFAULT_LOSSES)
+        wrap = DataParallelWithCallback(model, device_ids=[0])
+        optG, optD = model.create_optimizers(model.opt)
+        legs[name] = (wrap, optG, optD)
+    for r in range(a.rounds):
+        for name, (wrap, optG, optD) in legs.items():
+            if r == 0:
+                timed(lambda: train_iteration(wrap, optG, optD, dict(dev)), 1, warmup=2)
+            t = timed(lambda: [train_iteration(wrap, optG, optD, dict(dev)) for _ in range(a.steps)], 1, warmup=0)
+            res.setdefault("train_step_ms/" + name, []).append(t / a.steps)
+            print("round %d  %-26s train step %.1f ms  %.2f images/s" % (r, name, t / a.steps, 1e3 * n * a.steps / t))
+    del legs, wrap, optG, optD, model
+
+    crit = VGGLoss(make_opt(), state_dict=vgg19_state_dict(0))
+    g = torch.Generator().manual_seed(0)
+    fake, real, ref = [(torch.rand(n, 3, SIZE, SIZE, generator=g) * 2 - 1).cuda() for _ in range(3)]
+    lab_tag, lab_ref = (dev["label_tag"] == 1).float(), (dev["label_ref"] == 1).float()      # the hair class
+
+    def combined(masked):
+        x = fake.detach().requires_grad_()
+        kw = dict(label=lab_tag, style_label=lab_ref) if masked else {}
+        sum(vgg_objective(crit.vgg, x, real, ref, l1=True, content=True, style=True, **kw)).backward()
+
+    for r in range(a.rounds):
+        for key, masked in (("unmasked", False), ("remove_background", True)):
+            ms = timed(lambda: combined(masked), 5)
+            res.setdefault("vgg_default_ref_ne_tag_ms/" + key, []).append(ms)
+            print("round %d  VGG + content + style fwd+bwd, ref != tag, %-18s %.2f ms" % (r, key, ms))
+    os.makedirs(a.out_dir, exist_ok=True)
+    with open(os.path.join(a.out_dir, "vgg_lab_time_remove_background.json"), "w") as f:
         json.dump(res, f, indent=1)
 
 
