@@ -330,7 +330,8 @@ int mg_hole_mask(const float* mask, const float* orient_mask, const float* th_u,
 int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, int w, float wide_edge, void* stream);
 /* One launch for all terms of a loss evaluation.  terms_dev: device array of n_terms records of mg_loss_term_bytes()
  * bytes each, layout {const float* a; const float* b; float* ga; long long n; float scale, sign; int op, out_slot;
- * float target; int den_slot; const float* label; long long label_ns; int C, h, w, H, W, channels_last; const float* add;}:
+ * float target; int den_slot; const float* label; long long label_ns; int C, h, w, H, W, channels_last; const float* add;
+ * const float* table;}:
  *   slots[out_slot] += scale * sum_i f(a_i, b_i)   (fp64 accumulation; caller zeroes `slots`)
  *   op 0: f = min(sign*a - 1, 0) * (b ? b_i : 1)   hinge, discriminator side (b = weight map)     loss.py:104-120
  *   op 1: f = a                                    generator hinge -mean(D(fake)), gan_mode 'w'     loss.py:123-124
@@ -347,6 +348,12 @@ int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, i
  *   op 10: masked channel moments (calc_mean_std_mask, loss.py:634-654), l binary: per (n, c) slots[out_slot + n*2C + c] +=
  *          sum l a and slots[out_slot + n*2C + C + c] += sum l a^2 (mg_in_stats' [N][2][C] layout, fp32 runs of at most 32
  *          elements, fp64 above; scale not applied), and per image slots[den_slot + n] += sum l over its pixels (once per pixel).
+ *   op 11: count-balanced Lab L1 (LabColorLoss with balance_Lab, loss.py:490-531): a = fake, b = real, both [N,3,h,w] NCHW;
+ *          n = N*h*w counts PIXELS; label = the [N,1,h,w] hair mask (rows contiguous, image n at label + n*label_ns); table =
+ *          E[256][256] fp32, the weight of the bins (ka, kb).  Per pixel, with the Lab of mg_lab_loss_fwd:
+ *          ka = int(clamp(a_real + 128, 0, 255)), kb = int(clamp(b_real + 128, 0, 255)), w = E[ka][kb] * l, 0 -> 1;
+ *          f = w |a_fake - a_real| + w |b_fake - b_real| (per-pixel fp32, summed in fp64).  ga covers all three channels:
+ *          ga = add + g w (sgn da d a_fake/d fake + sgn db d b_fake/d fake), sign(0) = 0.  table is null for every other op.
  * mg_loss_reduce_bwd writes ga_i = add_i + gslots[out_slot] * scale * df/da for every term with ga != null (add null: ga_i =
  * gslots[out_slot] * scale * df/da; add may alias ga; no two terms of one launch may write the same ga).  Torch's tie rules:
  * the binary min gives each side half, |.| has gradient 0 at 0; BCE: sigmoid(a) - target.  Op 9: df/da = 2 (a l - b l) l.
@@ -386,7 +393,7 @@ int mg_maxpool2_relu_bwd(const float* dpool, const float* a32, const void* a16, 
 int mg_relu_bwd16(const float* dy, const float* add, const float* a32, const void* a16, int a_fmt, float* dz32, void* dz16, long long n,
                   void* stream);
 
-/* ---- Lab colour loss (models/networks/loss.py:403-531 LabColorLoss, balance_Lab = False) ----------------------------------
+/* ---- Lab colour loss (models/networks/loss.py:403-531 LabColorLoss, balance_Lab = False; balanced: mg_loss_reduce op 11) ---
  * fake, real [N,3,H,W] in [-1,1].  Per pixel: rgb = (img+1)/2, xyz = M rgb / rowsum(M) (loss.py:441-460), f(t) = t^(1/3) if
  * t > 0.008856 else 7.787 t + 0.137931, a = 500 (f(X) - f(Y)), b = 200 (f(Y) - f(Z)) (loss.py:462-485).
  * fwd: sums[0] += sum |a_fake - a_real| + |b_fake - b_real| (fp64, caller zeroes) => loss = sums[0] / (2*N*H*W) (loss.py:523).
@@ -405,7 +412,8 @@ int mg_lab_loss_bwd(const float* fake_nchw, const float* real_nchw, const float*
  *   give the same bits.  avg = sum / (sum m, 0 -> 1); loss = mean over the N x 2 values |avg_f - avg_r| of a and b.
  * mg_hair_avg_lab_bwd: dfake = mask_fake * (T[n][0] da/dfake + T[n][1] db/dfake), T[n][j] = gscale[0] / (2N) sgn(avg_f - avg_r)
  *   / cnt_f formed on the device from `sums` (gscale: device float = upstream gradient); f' branch by branch as mg_lab_loss_bwd.
- *   real is detached: there is no d real. */
+ *   real is detached: there is no d real.  With balance_Lab the host forms each image's weight from `sums` and launches the
+ *   backward once per image (N = 1, pointers offset to the image), gscale = upstream gradient * w[n] / N. */
 int mg_hair_avg_lab_fwd(const float* fake_nchw, const float* real_nchw, const float* mask_fake, const float* mask_real, double* sums,
                         int N, int H, int W, void* stream);
 int mg_hair_avg_lab_bwd(const float* fake_nchw, const float* mask_fake, const double* sums, const float* gscale, float* dfake_nchw,

@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmichigan_sm90.so")
 SOURCES = ["mg_api.cu", "mg_igemm.cu", "mg_aux.cu", "mg_wgrad.cu", "mg_bwd.cu", "mg_segconv.cu", "mg_peer.cu", "mg_loss.cu", "mg_conv3x3.cu", "mg_synth.cu", "mg_orient.cu", "mg_attn.cu", "mg_vgg.cu"]  # missing files are skipped
-HEADERS = ["mg_ptx.cuh", "mg_internal.h", "mg_epilogue.cuh", os.path.join("..", "..", "include", "michigan_b200.h")]
+HEADERS = ["mg_ptx.cuh", "mg_internal.h", "mg_epilogue.cuh", "mg_lab.cuh", os.path.join("..", "..", "include", "michigan_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math=false",

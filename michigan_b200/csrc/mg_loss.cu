@@ -5,11 +5,12 @@
 // loss.py:163-175: 8x l1_loss), ~60 launches per iteration forward and as many backward.  Here:
 //   * mg_edge_weight      the wide-edge weight map of one discriminator scale (loss.py:60-78) in one kernel;
 //   * mg_loss_reduce      ALL terms of a loss evaluation (the GAN terms of every scale in every gan_mode, the eight
-//                         feature-matching L1 terms, masked or not) through one descriptor table: warp-shuffle + fp64 atomics
-//                         into the loss slots;
+//                         feature-matching L1 terms, masked or not, and the count-balanced Lab colour L1) through one
+//                         descriptor table: warp-shuffle + fp64 atomics into the loss slots;
 //   * mg_loss_reduce_bwd  the matching gradients, one launch for every tensor in the table.
 #include <cuda_runtime.h>
 #include "mg_internal.h"
+#include "mg_lab.cuh"
 
 namespace mg {
 
@@ -79,6 +80,11 @@ __global__ void edge_weight_kernel(const float* __restrict__ label, float* __res
 //         slots[den_slot + n] += sum l over the image's PIXELS (each pixel once, not once per channel)    (calc_mean_std_mask,
 //         loss.py:634-654).  Backward: b is a [N][3][C] fp32 table (mu', A, B) written by mg_style_loss_fwd's masked mode and
 //         f'(a) = l (A + B (a - mu')).  The labels are binary (a channel of the one-hot label map, nearest-resized), l^2 = l.
+//   op 11 count-balanced Lab L1 (LabColorLoss with balance_Lab, loss.py:490-531): a = fake, b = real, both [N,3,h,w] NCHW, n =
+//         N h w PIXELS, label = the [N,1,h,w] hair mask (rows contiguous, image n at label + n * label_ns), table = E[256][256].
+//         Per pixel: Lab of both images (mg_lab.cuh), ka = int(clamp(a_real + 128, 0, 255)), kb likewise from b_real,
+//         w = E[ka][kb] l with 0 -> 1; f = w |a_fake - a_real| + w |b_fake - b_real| (each product rounded to fp32, the
+//         per-pixel values summed in fp64).  Backward: ga (all three channels) = g w (sgn da  da/dfake + sgn db  db/dfake).
 struct LossTerm {
     const float* a;
     const float* b;      // op 0: weight map (nullable); ops 2, 3, 8: the other tensor
@@ -96,6 +102,8 @@ struct LossTerm {
     // appended for the accumulating backward (null for every term before it)
     const float* add;    // backward: ga = add + g f'(a) (may alias ga); null: ga = g f'(a).  No two terms of one launch may
                          // write the same ga.
+    // appended for op 11 (null for every other op)
+    const float* table;  // E[ka][kb], 256 x 256 fp32: the balance weight of the bins (a + 128, b + 128) of the real pixel
 };
 
 // grid.x blocks per term: terms range from 9 K (coarse logits) to 34 M elements (finest feature map) - enough blocks to saturate
@@ -205,6 +213,59 @@ __device__ __forceinline__ double block_sum(double acc, double* part) {
     return s;
 }
 
+// op 11 at pixel i: the Lab of fake (t, f of its xyz) and the signs of its a, b differences to real, and the pixel's weight w
+struct BalancedLabPixel {
+    float t[3], f[3];
+    float da, db, w;
+};
+
+__device__ __forceinline__ BalancedLabPixel balanced_lab_pixel(const LossTerm& t, long long i, long long hw) {
+    const long long n = i / hw, p = i - n * hw;
+    BalancedLabPixel px;
+    float tr[3], fr[3];
+    lab_xyz(t.a + (size_t)n * 3 * hw, (size_t)hw, (size_t)p, px.t);
+    lab_xyz(t.b + (size_t)n * 3 * hw, (size_t)hw, (size_t)p, tr);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { px.f[k] = lab_f(px.t[k]); fr[k] = lab_f(tr[k]); }
+    const float ar = 500.f * (fr[0] - fr[1]), br = 200.f * (fr[1] - fr[2]);
+    px.da = 500.f * (px.f[0] - px.f[1]) - ar;
+    px.db = 200.f * (px.f[1] - px.f[2]) - br;
+    // loss.py:508-513: m = (b, a) + 128 clamped to [0, 255], truncated; the table is indexed [a bin][b bin]
+    const int ka = (int)fminf(fmaxf(ar + 128.f, 0.f), 255.f), kb = (int)fminf(fmaxf(br + 128.f, 0.f), 255.f);
+    const float w = __fmul_rn(__ldg(t.table + ka * 256 + kb), __ldg(t.label + n * t.label_ns + p));
+    px.w = w == 0.f ? 1.f : w;                                        // loss.py:517
+    return px;
+}
+
+// tp: the term's record in global memory (a reference to the kernel's local copy would put that copy on the stack)
+__device__ __noinline__ void balanced_lab_term(const LossTerm* __restrict__ tp, double* __restrict__ slots, double* part) {
+    const LossTerm t = *tp;
+    const long long hw = (long long)t.h * t.w;
+    double acc = 0.0;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
+        const BalancedLabPixel px = balanced_lab_pixel(t, i, hw);
+        acc += (double)__fmul_rn(px.w, fabsf(px.da)) + (double)__fmul_rn(px.w, fabsf(px.db));
+    }
+    const double s = block_sum(acc, part);
+    if (threadIdx.x == 0) atomicAdd(slots + t.out_slot, s * (double)t.scale);
+}
+
+// inlined: a call would raise the whole backward kernel to 54 registers (35 inline)
+__device__ __forceinline__ void balanced_lab_term_bwd(const LossTerm& t, float g) {
+    const long long hw = (long long)t.h * t.w;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
+        const BalancedLabPixel px = balanced_lab_pixel(t, i, hw);
+        float v[3];
+        lab_ab_backprop(px.t, px.f, sgn(px.da), sgn(px.db), g * px.w, v, 1);
+        const long long n = i / hw, p = i - n * hw;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const size_t k = ((size_t)n * 3 + c) * hw + p;
+            t.ga[k] = t.add ? t.add[k] + v[c] : v[c];
+        }
+    }
+}
+
 __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __restrict__ terms, double* __restrict__ slots) {
     const LossTerm t = terms[blockIdx.y];
     if ((long long)blockIdx.x * blockDim.x >= t.n && blockIdx.x != 0) return;      // no element of this term falls to this block
@@ -212,6 +273,10 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
     float accf = 0.f;
     if (t.op == 10) {
         moments_term(t, slots);
+        return;
+    }
+    if (t.op == 11) {
+        balanced_lab_term(terms + blockIdx.y, slots, part);
         return;
     }
     if (t.op >= 4) {
@@ -256,13 +321,17 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
 }
 
 // ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * ([sign*a - 1 < 0] + [sign*a - 1 == 0] / 2);  op 1: 1;
-// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10: term_df.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
+// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10: term_df;  op 11: balanced_lab_term_bwd.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
 // gives each side half the gradient.  The masked ops' denominators are folded into gslot by the caller.  With t.add the
 // result is added to add_i (which may be ga itself: each element is read before the same thread writes it).
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
     const LossTerm t = terms[blockIdx.y];
     if (!t.ga) return;
     const float g = __ldg(gslots + t.out_slot) * t.scale;
+    if (t.op == 11) {
+        balanced_lab_term_bwd(t, g);
+        return;
+    }
     if (t.op >= 4) {
         const bool masked = t.op >= 6;
         const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;

@@ -7,13 +7,17 @@ without --remove_background), evaluated by the fused reduction kernels of csrc/m
   * the wide-edge weight map (loss.py:60-78) is one kernel per scale, cached per (label, size) within an iteration.
 
 The rest of the generator objective follows: the Gabor orientation loss, VGGLoss / StyleContentLoss (every VGG19 term from one
-pass, _VGGObjectiveFn), LabColorLoss, RGBBackgroundL1Loss and the rgb L1 (RGBL1Loss).
+pass, _VGGObjectiveFn), LabColorLoss and HairAvgLabLoss (with or without --balance_Lab), RGBBackgroundL1Loss and the rgb L1
+(RGBL1Loss).
 """
 import ctypes as C
+import os
 from collections import namedtuple
 
+import numpy as np
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from .. import _lib, ops
 
@@ -26,7 +30,9 @@ class _Term(C.Structure):
                 ("C", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
                 ("channels_last", C.c_int32),
                 # appended for the accumulating backward (null: ga is written, not accumulated)
-                ("add", C.c_void_p)]
+                ("add", C.c_void_p),
+                # appended for op 11 (null for every other op)
+                ("table", C.c_void_p)]
 
 
 OP_HINGE_D, OP_SUM, OP_L1, OP_SQ = 0, 1, 2, 3
@@ -34,6 +40,8 @@ OP_HINGE_D, OP_SUM, OP_L1, OP_SQ = 0, 1, 2, 3
 OP_BCE, OP_SQ_T, OP_WSUM, OP_HINGE_MASK, OP_L1_MASK = 4, 5, 6, 7, 8
 # --remove_background in VGGLoss / StyleContentLoss: the masked content term and the masked channel moments of one VGG tap
 OP_SQ_MASK, OP_MOMENTS = 9, 10
+# LabColorLoss with --balance_Lab: the Lab L1 weighted per pixel by the count table of the real pixel's (a, b) bins
+OP_LAB_BALANCED = 11
 MASKED_OPS = (OP_WSUM, OP_HINGE_MASK, OP_L1_MASK, OP_SQ_MASK)      # one scalar term over its own sum(label1) * c + 1e-5
 DEN_EPS = 1e-5          # loss.py:111, 114, 117, 160, 196, 677: sum(label1) * c + 1e-5
 _table_cache = {}
@@ -677,6 +685,61 @@ class RGBL1Loss(nn.Module):
         return _PixelL1Fn.apply(fake, image_tag.float(), None)
 
 
+LAB_WEIGHT_TH = 10.0        # train_options.py:78, the default --Lab_weight_th
+_lab_weight_cache = {}
+
+
+def balanced_lab(opt, who):
+    """Whether `who` (LabColorLoss, HairAvgLabLoss) computes the count-balanced loss of --balance_Lab (loss.py:490-531,
+    578-621): opt.balance_Lab set and opt.weight_dir naming the count table.  The reference's option parser always provides
+    weight_dir (train_options.py:77), so its train.py --balance_Lab runs balanced under install().  balance_Lab without
+    weight_dir is refused with NotImplementedError, as before the balanced loss existed."""
+    if not getattr(opt, "balance_Lab", False):
+        return False
+    if getattr(opt, "weight_dir", None) is None:
+        raise NotImplementedError("michigan_b200: %s with --balance_Lab needs opt.weight_dir, the [256,256] colour-count table "
+                                  "(the reference's train options provide it: --weight_dir, default ./data/ab_count.npy)" % who)
+    return True
+
+
+def lab_weight_table(path, th=LAB_WEIGHT_TH, device="cpu"):
+    """E[ka][kb] ([256,256] fp32 on `device`): the weight cal_weight (loss.py:487-513, 578-597) looks up for a pixel whose real a
+    and b fall in the bins ka = int(clamp(a + 128, 0, 255)) and kb likewise.
+
+    The count table T = np.load(path) is processed with the reference's fp32 torch operations (T == 0 -> 1, max(T) / T,
+    clamped at th), then torch's own grid_sample (mode 'nearest', align_corners False, zero padding) is run once on the grid
+    of all (ka, kb) bins, so E matches the reference's lookup bit for bit, including the bins its grid maps outside the
+    table (bin 255 reads 0).  The reference reads the file on every forward; here it is read once per (path, th) and E is
+    kept per (path, th, device)."""
+    key = (os.path.realpath(path), float(th))
+    dev = torch.device(device)
+    hit = _lab_weight_cache.get(key + (dev,))
+    if hit is not None:
+        return hit
+    cpu = _lab_weight_cache.get(key + (torch.device("cpu"),))
+    if cpu is None:
+        if not os.path.isfile(path):
+            raise FileNotFoundError("--balance_Lab: colour-count table %s not found (--weight_dir)" % path)
+        raw = np.load(path)
+        if raw.shape != (256, 256):
+            raise ValueError("--balance_Lab: the colour-count table %s must be [256,256], got %s" % (path, tuple(raw.shape)))
+        w = torch.tensor(raw, dtype=torch.float32).view(1, 1, 256, 256)     # self.FloatTensor(raw)
+        w[w == 0] = 1
+        w = w.max() / w
+        w[w > th] = th
+        m = (torch.arange(256, dtype=torch.float32) - 127.5) / 127.5          # (m - 127.5) / 127.5 on the integer bins
+        grid = torch.stack([m.view(1, 256).expand(256, 256), m.view(256, 1).expand(256, 256)], -1).unsqueeze(0)  # (b, a)
+        cpu = F.grid_sample(w, grid, mode="nearest", padding_mode="zeros", align_corners=False)[0, 0].contiguous()
+        _lab_weight_cache[key + (torch.device("cpu"),)] = cpu
+    hit = cpu.to(dev)
+    _lab_weight_cache[key + (dev,)] = hit
+    return hit
+
+
+def _lab_table_key(opt):
+    return opt.weight_dir, float(getattr(opt, "Lab_weight_th", LAB_WEIGHT_TH))
+
+
 class _LabLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, fake, real):
@@ -693,48 +756,117 @@ class _LabLossFn(torch.autograd.Function):
         return ops.lab_loss_bwd(f, r, gscale), None
 
 
+def _balanced_lab_term(f, r, mask, table, ga):
+    """The op 11 record of fake f and real r ([N,3,H,W] contiguous), mask [N,1,H,W] (rows contiguous), E on the device."""
+    n, _, h, w = f.shape
+    t = _Term(f.data_ptr(), r.data_ptr(), ga.data_ptr() if ga is not None else None, n * h * w, 1.0, 1.0, OP_LAB_BALANCED, 0)
+    t.label, t.label_ns = mask.data_ptr(), mask.stride(0)
+    t.C, t.h, t.w, t.H, t.W = 3, h, w, h, w
+    t.table = table.data_ptr()
+    return t
+
+
+class _BalancedLabFn(torch.autograd.Function):
+    """mean(w * |ab_fake - ab_real|) over N x 2 x H x W: one mg_loss_reduce launch of op 11 each way."""
+
+    @staticmethod
+    def forward(ctx, fake, real, mask, table):
+        assert _lib.load().mg_loss_term_bytes() == C.sizeof(_Term)
+        f, r = fake.detach().contiguous(), real.detach().contiguous()
+        slots = torch.zeros(1, device=f.device, dtype=torch.float64)
+        terms = _device_table([_balanced_lab_term(f, r, mask, table, None)], f.device)
+        _lib.check(_lib.load().mg_loss_reduce(terms.data_ptr(), 1, slots.data_ptr(), ops._stream()), "mg_loss_reduce")
+        ctx.save_for_backward(f, r, mask, table)
+        ctx.count = 2 * f.shape[0] * f.shape[2] * f.shape[3]
+        return (slots / ctx.count).float().reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        f, r, mask, table = ctx.saved_tensors
+        ga = torch.empty_like(f)
+        gslot = (g.double() / ctx.count).float().reshape(1).contiguous()
+        terms = _device_table([_balanced_lab_term(f, r, mask, table, ga)], f.device)
+        _lib.check(_lib.load().mg_loss_reduce_bwd(terms.data_ptr(), 1, gslot.data_ptr(), ops._stream()), "mg_loss_reduce_bwd")
+        return ga, None, None, None
+
+
 class LabColorLoss(nn.Module):
-    """loss.py:403-531 with balance_Lab=False: L1 between the a, b channels of the Lab images of fake and real.detach()
-    (xyz2lab of rgb2xyz((img + 1) / 2)), one fused kernel each way (csrc/mg_vgg.cu)."""
+    """loss.py:403-531: L1 between the a, b channels of the Lab images of fake and real.detach() (xyz2lab of
+    rgb2xyz((img + 1) / 2)), one fused kernel each way (csrc/mg_vgg.cu).
+
+    With --balance_Lab and opt.weight_dir (balanced_lab) it is the count-balanced loss mean(w * |ab_fake - ab_real|), w per
+    pixel = E[bins of the real pixel's a, b] * mask with 0 -> 1 (lab_weight_table; mask = the tag's hair, [N,1,H,W]), on
+    mg_loss_reduce op 11 each way.  The count table is read once, at construction."""
 
     def __init__(self, opt):
         super().__init__()
-        if getattr(opt, "balance_Lab", False):
-            raise NotImplementedError("michigan_b200: --balance_Lab is not implemented (it needs data/ab_count.npy and grid_sample)")
         self.opt = opt
+        self.table_key = None
+        if balanced_lab(opt, "LabColorLoss"):
+            self.table_key = _lab_table_key(opt)
+            lab_weight_table(*self.table_key)
 
     def forward(self, fake, real, mask=None):
         if fake.shape != real.shape or fake.shape[1] != 3:
             raise ValueError("LabColorLoss: expected two [N,3,H,W] images, got %s and %s" % (tuple(fake.shape), tuple(real.shape)))
-        return _LabLossFn.apply(fake, real.float())
+        if self.table_key is None:
+            return _LabLossFn.apply(fake, real.float())
+        n, _, h, w = fake.shape
+        if mask is None or tuple(mask.shape) != (n, 1, h, w):
+            raise ValueError("LabColorLoss: --balance_Lab needs the hair mask [N,1,H,W] = %s, got %s"
+                             % ((n, 1, h, w), None if mask is None else tuple(mask.shape)))
+        table = lab_weight_table(*self.table_key, device=fake.device)
+        return _BalancedLabFn.apply(fake, real.float(), _hair_label(mask, fake), table)
 
 
 class _HairAvgLabFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, fake, real, mask_fake, mask_real):
+    def forward(ctx, fake, real, mask_fake, mask_real, table):
         f, mf = fake.detach().contiguous(), mask_fake.detach().contiguous()
         sums = ops.hair_avg_lab_fwd(f, real.detach().contiguous(), mf, mask_real.detach().contiguous())
         ctx.save_for_backward(f, mf, sums)
         cnt = sums[:, :, 3:]
         avg = sums[:, :, 1:3] / torch.where(cnt == 0, torch.ones_like(cnt), cnt)       # loss.py:575
-        return (avg[:, 0] - avg[:, 1]).abs().mean().float()
+        diff = (avg[:, 0] - avg[:, 1]).abs()
+        ctx.w = None
+        if table is None:
+            return diff.mean().float()
+        # loss.py:589-597 on the real averages (fp32, as the reference holds them): N gathers, no host synchronisation
+        k = (avg[:, 1].float() + 128).clamp(0, 255).int().long()
+        ctx.w = table[k[:, 0], k[:, 1]]
+        return (diff * ctx.w.double().unsqueeze(1)).mean().float()
 
     @staticmethod
     def backward(ctx, g):
         f, mf, sums = ctx.saved_tensors
-        return ops.hair_avg_lab_bwd(f, mf, sums, g.float().reshape(1).contiguous()), None, None, None
+        if ctx.w is None:
+            return ops.hair_avg_lab_bwd(f, mf, sums, g.float().reshape(1).contiguous()), None, None, None, None
+        # image n's gradient is the unbalanced one of a batch of 1 scaled by w[n] / N: one launch per image
+        n = f.shape[0]
+        gs = (g.double() * ctx.w.double() / n).float().contiguous()
+        dfake = torch.empty_like(f)
+        for i in range(n):
+            ops.hair_avg_lab_bwd(f[i:i + 1], mf[i:i + 1], sums[i:i + 1], gs[i:i + 1], out=dfake[i:i + 1])
+        return dfake, None, None, None, None
 
 
 class HairAvgLabLoss(nn.Module):
-    """loss.py:534-621 with balance_Lab=False: L1 between the hair-averaged a, b of fake (tag hair mask_fake) and of
-    real.detach() (reference hair mask_real), avg = sum(Lab * m) / sum(m), a mask sum of 0 counted as 1.  One fused kernel
-    pair each way (csrc/mg_vgg.cu: mg_hair_avg_lab_fwd, mg_hair_avg_lab_bwd)."""
+    """loss.py:534-621: L1 between the hair-averaged a, b of fake (tag hair mask_fake) and of real.detach() (reference hair
+    mask_real), avg = sum(Lab * m) / sum(m), a mask sum of 0 counted as 1.  One fused kernel pair each way (csrc/mg_vgg.cu:
+    mg_hair_avg_lab_fwd, mg_hair_avg_lab_bwd).
+
+    With --balance_Lab and opt.weight_dir (balanced_lab): mean(w[n] * |avg_ab_fake - avg_ab_real|), w[n] = E[bins of image n's
+    real average a, b] (lab_weight_table; no mask factor, no 0 -> 1), gathered on the device from the forward's sums; the
+    backward runs mg_hair_avg_lab_bwd once per image with the gradient scaled by w[n].  The count table is read once, at
+    construction."""
 
     def __init__(self, opt):
         super().__init__()
-        if getattr(opt, "balance_Lab", False):
-            raise NotImplementedError("michigan_b200: --balance_Lab is not implemented (it needs data/ab_count.npy and grid_sample)")
         self.opt = opt
+        self.table_key = None
+        if balanced_lab(opt, "HairAvgLabLoss"):
+            self.table_key = _lab_table_key(opt)
+            lab_weight_table(*self.table_key)
 
     def forward(self, fake, real, mask_fake, mask_real):
         if fake.shape != real.shape or fake.shape[1] != 3:
@@ -743,7 +875,8 @@ class HairAvgLabLoss(nn.Module):
         for name, m in (("mask_fake", mask_fake), ("mask_real", mask_real)):
             if tuple(m.shape) != (n, 1, h, w):
                 raise ValueError("HairAvgLabLoss: %s must be [N,1,H,W] = %s, got %s" % (name, (n, 1, h, w), tuple(m.shape)))
-        return _HairAvgLabFn.apply(fake, real.float(), mask_fake.float(), mask_real.float())
+        table = None if self.table_key is None else lab_weight_table(*self.table_key, device=fake.device)
+        return _HairAvgLabFn.apply(fake, real.float(), mask_fake.float(), mask_real.float(), table)
 
 
 class L1OLoss(nn.Module):

@@ -696,11 +696,15 @@ def hair_avg_lab_fwd(fake, real, mask_fake, mask_real):
     return sums
 
 
-def hair_avg_lab_bwd(fake, mask_fake, sums, g):
-    """d fake [N,3,H,W] of g[0] * the hair-average Lab loss given hair_avg_lab_fwd's sums; g: [1] fp32 device tensor."""
+def hair_avg_lab_bwd(fake, mask_fake, sums, g, out=None):
+    """d fake [N,3,H,W] of g[0] * the hair-average Lab loss given hair_avg_lab_fwd's sums; g: [1] fp32 device tensor; out: a
+    contiguous [N,3,H,W] fp32 tensor to write it into (default: a new one)."""
     _chk(fake, "fake"); _chk(mask_fake, "mask_fake"); _chk(sums, "sums", torch.float64); _chk(g, "g")
     N, _, H, W = fake.shape
-    dfake = torch.empty_like(fake)
+    dfake = torch.empty_like(fake) if out is None else out
+    if out is not None:
+        _chk(out, "out")
+        assert out.shape == fake.shape, (out.shape, fake.shape)
     check(_lib.load().mg_hair_avg_lab_bwd(_p(fake), _p(mask_fake), _p(sums), _p(g), _p(dfake), N, H, W, _stream()),
           "mg_hair_avg_lab_bwd")
     return dfake

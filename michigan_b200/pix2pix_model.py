@@ -35,7 +35,7 @@ class Pix2PixModel(torch.nn.Module):
         # (any --gan_mode), GAN_Feat, VGG, content, style, background, rgb, lab, ORIENT, CONFIDENCE, each dropped by its --no_*
         # flag.  GANLoss and GANFeatLoss take --remove_background; VGGLoss and StyleContentLoss take it together with
         # mask_vgg_losses (the reference's hair-masked terms, networks.loss.masked_vgg_losses) and refuse it alone; LabColorLoss
-        # refuses --balance_Lab.
+        # takes --balance_Lab when opt.weight_dir names the count table (networks.loss.balanced_lab) and refuses it without.
         self.netIG = None
         if getattr(opt, "use_ig", False):
             self.netIG = networks.define_IG(opt)
