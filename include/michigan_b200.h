@@ -141,6 +141,16 @@ typedef struct mg_thin_args {
     void* out_hi;
     void* out_lo;
     int32_t out16_fmt;
+    /* arg-max epilogue: the Difference-of-Gaussians orientation response of L1OLoss (loss.py:320-340), selected by
+     * argmax_idx != null (all three null for every other conv).  in = the [N,3,H,W] NCHW image in [-1,1], read as its gray
+     * 0.299 R + 0.587 G + 0.144 B of (x+1)/2*255 (loss.py:357-358); w = the [17*17][32] bank (filter index fastest); CinP 3,
+     * Cout 32, KH = KW = 17, stride 1, zero pad 8, OH = H, OW = W; bias, pscale, pmul, act, round_out, seg_resize and the
+     * 16-bit copies unset.  Per pixel r = max_k max(conv_k, 0) in exact fp32, argmax_idx [N,H,W] uint8 = its first arg-max,
+     * out [N,H,W] = r * argmax_mask[n,y,x] (fp32 product); *argmax_max (caller zeroes) = the maximum of out over the whole
+     * call, folded in with an integer atomicMax on the bits of the non-negative floats (no host synchronisation). */
+    void* argmax_idx;
+    const float* argmax_mask;
+    float* argmax_max;
 } mg_thin_args;
 int mg_conv_thin(const mg_thin_args* a, void* stream);
 int mg_pack_weight_thin(const float* w_oihw, float* wt, int O, int I, int CinP, int KH, int KW, void* stream);
@@ -331,7 +341,7 @@ int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, i
 /* One launch for all terms of a loss evaluation.  terms_dev: device array of n_terms records of mg_loss_term_bytes()
  * bytes each, layout {const float* a; const float* b; float* ga; long long n; float scale, sign; int op, out_slot;
  * float target; int den_slot; const float* label; long long label_ns; int C, h, w, H, W, channels_last; const float* add;
- * const float* table;}:
+ * const float* table; const unsigned char* idx; const float* maxv;}:
  *   slots[out_slot] += scale * sum_i f(a_i, b_i)   (fp64 accumulation; caller zeroes `slots`)
  *   op 0: f = min(sign*a - 1, 0) * (b ? b_i : 1)   hinge, discriminator side (b = weight map)     loss.py:104-120
  *   op 1: f = a                                    generator hinge -mean(D(fake)), gan_mode 'w'     loss.py:123-124
@@ -354,6 +364,16 @@ int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, i
  *          ka = int(clamp(a_real + 128, 0, 255)), kb = int(clamp(b_real + 128, 0, 255)), w = E[ka][kb] * l, 0 -> 1;
  *          f = w |a_fake - a_real| + w |b_fake - b_real| (per-pixel fp32, summed in fp64).  ga covers all three channels:
  *          ga = add + g w (sgn da d a_fake/d fake + sgn db d b_fake/d fake), sign(0) = 0.  table is null for every other op.
+ *   op 12: DoG orientation and confidence losses (L1OLoss with an orient_filter other than 'gabor', loss.py:320-385): a = rh
+ *          [N,h,w] and maxv = its batch maximum M and idx = the arg-max filters, as the arg-max epilogue of mg_conv_thin wrote
+ *          them; b = label2 [N,2,h,w] (sin 2t, cos 2t of the target); label = hair [N,h,w] contiguous; table = [2][32] fp32 sin
+ *          and cos of 2 (k pi / 32); n = N*h*w PIXELS (< 2^31).  Per pixel conf = rh / M (IEEE division), 0 where <= 0;
+ *          (s, c) = table[.][idx]; ds = s conf hair - ls hair, dc likewise, dcf = conf hair - hair.  Six slots from out_slot:
+ *          sum |ds| + |dc|, sum |dcf|, sum hair, sum Lo (-rh / M^2), sum Lc (-rh / M^2), #{rh == M}, with Lo = [conf > 0] hair
+ *          (sgn ds s + sgn dc c) and Lc = [conf > 0] hair sgn dcf (fp32 per thread, fp64 across threads).  M = 0 gives NaN.
+ *          Backward: gslots[out_slot + 0..2] = (go, gc, share), share = (go slot3 + gc slot4) / slot5 formed by the caller;
+ *          ga = dL/dr = hair ((go Lo + gc Lc) / M + [rh == M] share) (add is not applied).  idx and maxv are null for every
+ *          other op.
  * mg_loss_reduce_bwd writes ga_i = add_i + gslots[out_slot] * scale * df/da for every term with ga != null (add null: ga_i =
  * gslots[out_slot] * scale * df/da; add may alias ga; no two terms of one launch may write the same ga).  Torch's tie rules:
  * the binary min gives each side half, |.| has gradient 0 at 0; BCE: sigmoid(a) - target.  Op 9: df/da = 2 (a l - b l) l.
@@ -362,7 +382,8 @@ int mg_loss_reduce(const void* terms_dev, int n_terms, double* slots, void* stre
 int mg_loss_reduce_bwd(const void* terms_dev, int n_terms, const float* gslots, void* stream);
 int mg_loss_term_bytes(void);
 
-/* ---- Gabor orientation loss (models/networks/loss.py:274-385 L1OLoss, orient_filter 'gabor') --------------------------------
+/* ---- Gabor orientation loss (models/networks/loss.py:274-385 L1OLoss, orient_filter 'gabor'; the DoG variant is the arg-max
+ * epilogue of mg_conv_thin, mg_loss_reduce op 12 and mg_orient_loss_bwd with the DoG bank, weights2 = {1, 0}) -----------------
  * img [N,3,H,W] in [-1,1]; bank [17*17][32] = the 32 Gabor kernels of gabor_fn (loss.py:214-240), filter index fastest;
  * label2 [N,2,H,W] = (sin 2t, cos 2t) of the target orientation; hair [N,H,W].
  * fwd: sums[0] += sum |orient_fake*hair - label2*hair| (both channels), sums[1] += sum log(clamp(conf,.001,1))*hair,

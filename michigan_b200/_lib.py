@@ -47,6 +47,7 @@ class ThinArgs(C.Structure):
         ("act", C.c_int32), ("round_out", C.c_int32),
         ("pscale", c_f32p), ("pmul", c_f32p),
         ("out_hi", c_f32p), ("out_lo", c_f32p), ("out16_fmt", C.c_int32),
+        ("argmax_idx", c_f32p), ("argmax_mask", c_f32p), ("argmax_max", c_f32p),
     ]
 
 

@@ -947,6 +947,7 @@ extern "C" int mg_pack_weight_thin(const float* w, float* wt, int O, int I, int 
 }
 
 extern "C" int mg_conv_thin(const mg_thin_args* a, void* stream) {
+    if (a && a->argmax_idx && a->in && a->w) return orient_argmax_conv(a, ST(stream));
     if (!a || !a->in || !a->w || (!a->out && !a->out_hi)) return set_error(-1, "mg_conv_thin: null pointer");
     if (a->out_hi && (a->out16_fmt < 1 || a->out16_fmt > 2)) return set_error(-6, "mg_conv_thin: out16_fmt must be 1 or 2");
     if (a->CinP != 4 && a->CinP != 8) return set_error(-2, "mg_conv_thin: CinP must be 4 or 8");

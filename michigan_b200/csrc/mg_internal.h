@@ -46,6 +46,9 @@ int probe_bits();   // env MG_DBG, read once
 #define MG_PROFV(p) 0
 #endif
 
+// mg_orient.cu: mg_conv_thin with argmax_idx set (the DoG orientation response and its batch maximum)
+int orient_argmax_conv(const mg_thin_args* a, cudaStream_t stream);
+
 struct IgemmParams;
 // mg_conv3x3.cu: 1 = launched, 0 = shape not eligible (use the per-tap kernel), anything else = error status
 int conv3x3_group_launch(const mg_igemm_args* a, IgemmParams& p, int BN, int cw, int scratch_bytes, int spec, cudaStream_t stream);

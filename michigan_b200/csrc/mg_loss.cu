@@ -85,6 +85,18 @@ __global__ void edge_weight_kernel(const float* __restrict__ label, float* __res
 //         Per pixel: Lab of both images (mg_lab.cuh), ka = int(clamp(a_real + 128, 0, 255)), kb likewise from b_real,
 //         w = E[ka][kb] l with 0 -> 1; f = w |a_fake - a_real| + w |b_fake - b_real| (each product rounded to fp32, the
 //         per-pixel values summed in fp64).  Backward: ga (all three channels) = g w (sgn da  da/dfake + sgn db  db/dfake).
+//   op 12 DoG orientation and confidence losses (L1OLoss, orient_filter not 'gabor', loss.py:320-385): a = rh = r * hair of
+//         the response pass (mg_conv_thin's arg-max epilogue), idx its arg-max, maxv its batch maximum M, b = label2 [N,2,h,w]
+//         (sin 2t, cos 2t of the target), label = hair [N,h,w] contiguous, n = N h w PIXELS (< 2^31).  Per pixel
+//         conf = rh / M (IEEE division: exactly 1 at the maximiser), 0 where conf <= 0; (s, c) = table[0][idx], table[1][idx],
+//         the caller's (sin, cos) of 2 (k pi / 32) (loss.py:345-348, formed by torch as the reference does);
+//         ds = s conf hair - ls hair, dc likewise, dcf = conf hair - hair.  Six fp64 slots from out_slot:
+//           [0] sum |ds| + |dc|   [1] sum |dcf|   [2] sum hair
+//           [3] sum Lo (-rh / M^2), [4] sum Lc (-rh / M^2): the derivatives through M, Lo = [conf > 0] hair (sgn ds s + sgn dc c)
+//               and Lc = [conf > 0] hair sgn dcf the per-pixel d/dconf of [0] and [1]
+//           [5] the number of pixels with rh == M (torch splits the gradient of a max evenly among ties).
+//         Backward, gslots[out_slot + 0..2] = (go, gc, share) with share = (go [3] + gc [4]) / [5] (formed by the caller):
+//         ga = dL/dr = hair ((go Lo + gc Lc) / M + (rh == M ? share : 0)).
 struct LossTerm {
     const float* a;
     const float* b;      // op 0: weight map (nullable); ops 2, 3, 8: the other tensor
@@ -104,6 +116,9 @@ struct LossTerm {
                          // write the same ga.
     // appended for op 11 (null for every other op)
     const float* table;  // E[ka][kb], 256 x 256 fp32: the balance weight of the bins (a + 128, b + 128) of the real pixel
+    // appended for op 12 (null for every other op)
+    const unsigned char* idx;  // [N,h,w] arg-max filter k of each pixel (op 12's table: [2][32] fp32, sin and cos of 2 (k pi / 32))
+    const float* maxv;         // the batch maximum M of a (one float)
 };
 
 // grid.x blocks per term: terms range from 9 K (coarse logits) to 34 M elements (finest feature map) - enough blocks to saturate
@@ -266,6 +281,67 @@ __device__ __forceinline__ void balanced_lab_term_bwd(const LossTerm& t, float g
     }
 }
 
+// op 12 at pixel i (n < 2^31 pixels, checked by the caller): rh, hair, and the per-pixel d/dconf of the orientation and
+// confidence sums (zero where conf <= 0); with kSums also |ds| + |dc| and |dcf|.  hair is read as label[i] (label_ns = h w).
+struct DogPixel {
+    float rh, h, lo, lc, fo, fc;
+};
+
+template <bool kSums>
+__device__ __forceinline__ DogPixel dog_pixel(const LossTerm& t, int i, int hw, float M) {
+    const int n = i / hw;
+    DogPixel px;
+    px.rh = __ldg(t.a + i);
+    px.h = __ldg(t.label + i);
+    const float q = px.rh / M;                                    // loss.py:341 (IEEE: no reciprocal)
+    const bool pos = q > 0.f || q != q;                           // loss.py:342-343: conf * (1 - [conf <= 0])
+    const float conf = pos ? q : 0.f;
+    const int k = __ldg(t.idx + i);
+    const float s = __ldg(t.table + k), c = __ldg(t.table + 32 + k);
+    const float* lab = t.b + (size_t)i + (size_t)n * hw;          // label2[n, 0, p], p = i - n hw
+    const float ds = __fmul_rn(__fmul_rn(s, conf), px.h) - __fmul_rn(__ldg(lab), px.h);
+    const float dc = __fmul_rn(__fmul_rn(c, conf), px.h) - __fmul_rn(__ldg(lab + hw), px.h);
+    const float dcf = __fmul_rn(conf, px.h) - px.h;
+    px.lo = pos ? (sgn(ds) * s + sgn(dc) * c) * px.h : 0.f;
+    px.lc = pos ? sgn(dcf) * px.h : 0.f;
+    if (kSums) { px.fo = fabsf(ds) + fabsf(dc); px.fc = fabsf(dcf); }
+    return px;
+}
+
+// tp: the term's record in global memory (as balanced_lab_term).  fp32 partials per thread, fp64 across threads.
+__device__ __noinline__ void dog_orient_term(const LossTerm* __restrict__ tp, double* __restrict__ slots, double* part) {
+    const LossTerm t = *tp;
+    const int hw = t.h * t.w;
+    const float M = __ldg(t.maxv);
+    float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (int)t.n; i += gridDim.x * blockDim.x) {
+        const DogPixel px = dog_pixel<true>(t, i, hw, M);
+        const float dm = -(px.rh / M) / M;                        // d conf / d M before the [conf > 0] factor
+        acc[0] += px.fo;
+        acc[1] += px.fc;
+        acc[2] += px.h;
+        acc[3] += px.lo * dm;
+        acc[4] += px.lc * dm;
+        acc[5] += px.rh == M ? 1.f : 0.f;
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        if (k) __syncthreads();
+        const double s = block_sum((double)acc[k], part);
+        if (threadIdx.x == 0) atomicAdd(slots + t.out_slot + k, s);
+    }
+}
+
+__device__ __forceinline__ void dog_orient_term_bwd(const LossTerm& t, const float* __restrict__ gslots) {
+    const int hw = t.h * t.w;
+    const float M = __ldg(t.maxv);
+    const float go = __ldg(gslots + t.out_slot), gc = __ldg(gslots + t.out_slot + 1), share = __ldg(gslots + t.out_slot + 2);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (int)t.n; i += gridDim.x * blockDim.x) {
+        const DogPixel px = dog_pixel<false>(t, i, hw, M);
+        t.ga[i] = px.h * ((go * px.lo + gc * px.lc) / M + (px.rh == M ? share : 0.f));
+    }
+}
+
 __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __restrict__ terms, double* __restrict__ slots) {
     const LossTerm t = terms[blockIdx.y];
     if ((long long)blockIdx.x * blockDim.x >= t.n && blockIdx.x != 0) return;      // no element of this term falls to this block
@@ -277,6 +353,10 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
     }
     if (t.op == 11) {
         balanced_lab_term(terms + blockIdx.y, slots, part);
+        return;
+    }
+    if (t.op == 12) {
+        dog_orient_term(terms + blockIdx.y, slots, part);
         return;
     }
     if (t.op >= 4) {
@@ -321,7 +401,7 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
 }
 
 // ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * ([sign*a - 1 < 0] + [sign*a - 1 == 0] / 2);  op 1: 1;
-// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10: term_df;  op 11: balanced_lab_term_bwd.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
+// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10: term_df;  op 11: balanced_lab_term_bwd;  op 12: dog_orient_term_bwd.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
 // gives each side half the gradient.  The masked ops' denominators are folded into gslot by the caller.  With t.add the
 // result is added to add_i (which may be ga itself: each element is read before the same thread writes it).
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
@@ -330,6 +410,10 @@ __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __
     const float g = __ldg(gslots + t.out_slot) * t.scale;
     if (t.op == 11) {
         balanced_lab_term_bwd(t, g);
+        return;
+    }
+    if (t.op == 12) {
+        dog_orient_term_bwd(t, gslots);
         return;
     }
     if (t.op >= 4) {

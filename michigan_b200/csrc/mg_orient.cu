@@ -1,5 +1,5 @@
-// michigan_b200 — Gabor orientation loss (SURVEY.md §8f row 2, first slice; reference models/networks/loss.py:274-385 L1OLoss,
-// orient_filter = 'gabor').
+// michigan_b200 — orientation losses (SURVEY.md §8f row 2; reference models/networks/loss.py:274-385 L1OLoss, orient_filter
+// 'gabor' and the Difference-of-Gaussians variant).
 //
 // The reference builds 32 17x17 Gabor kernels ON THE FLY every call (gabor_fn, loss.py:214-240), runs 32 separate
 // 1 -> 1 channel conv2d launches on the gray image, concatenates, clamps, arg-maxes, and evaluates two masked reductions:
@@ -9,6 +9,11 @@
 //              loss sums reduced with warp shuffles + fp64 atomics; writes per pixel the winning filter index and dL/d(response);
 //   backward : one gather kernel - d gray[q] = sum over the 17x17 neighbours p of g[p] * K_{idx[p]}[q - p], then the RGB
 //              coefficients (loss.py:338-340, including the reference's 0.144 blue weight).
+// The DoG variant (loss.py:320-349) normalises every confidence by ONE maximum over the batch, so its forward is two-pass:
+//   response : dog_response_kernel (mg_conv_thin with argmax_idx set) - the same tile and accumulators, then per pixel the first
+//              arg-max, r * hair and an integer atomicMax of its bits into the batch maximum M;
+//   loss     : mg_loss_reduce op 12 (mg_loss.cu) - conf = r hair / M, both loss sums and the M-path sums of the backward;
+//   backward : mg_loss_reduce_bwd op 12 writes dL/dr, then orient_bwd_kernel above gathers it through the DoG bank.
 #include <cuda_runtime.h>
 #include "mg_internal.h"
 
@@ -22,6 +27,29 @@ __device__ __forceinline__ float gray_of(const float* img, size_t plane, size_t 
     // loss.py:338-340: fake = (x+1)/2*255; gray = 0.299 R + 0.587 G + 0.144 B
     const float r = (img[off] + 1.f) * 0.5f * 255.f, g = (img[plane + off] + 1.f) * 0.5f * 255.f, b = (img[2 * plane + off] + 1.f) * 0.5f * 255.f;
     return 0.299f * r + 0.587f * g + 0.144f * b;
+}
+
+// The gray tile + halo of the 16 x 16 output tile at (y0, x0) of one image (im = its [3,H,W] planes), zero outside the image.
+// The helpers shared by the forward kernels take the calling kernel as a template tag: an instantiation with one caller is
+// inlined before it is optimised on its own, which keeps orient_fwd_kernel's code exactly as it was before the DoG kernel
+// shared it.
+template <int kCaller>
+__device__ __forceinline__ void orient_stage_gray(const float* __restrict__ im, float* tile, int y0, int x0, int H, int W, size_t plane) {
+    for (int i = threadIdx.x; i < kOP * kOP; i += 256) {
+        const int ty = i / kOP, tx = i - ty * kOP;
+        const int y = y0 + ty - kOR, x = x0 + tx - kOR;
+        tile[ty * (kOP + 1) + tx] = (y >= 0 && y < H && x >= 0 && x < W) ? gray_of(im, plane, (size_t)y * W + x) : 0.f;
+    }
+}
+
+// resTensor[res < 0] = 0; max and argmax (first maximum) over the 32 clamped responses (loss.py:308-310, 335-337)
+template <int kCaller>
+__device__ __forceinline__ int orient_argmax(const float (&acc)[kOF], float& mx) {
+    int best = 0;
+    mx = fmaxf(acc[0], 0.f);
+#pragma unroll
+    for (int k = 1; k < kOF; ++k) { const float v = fmaxf(acc[k], 0.f); if (v > mx) { mx = v; best = k; } }
+    return best;
 }
 
 // bank: [17*17][32] (filter index fastest).  label2: [N,2,H,W] (sin 2t, cos 2t of the target orientation, un-masked).
@@ -43,11 +71,7 @@ __global__ void __launch_bounds__(256) orient_fwd_kernel(const float* __restrict
         const int y0 = (r / tiles_w) * kOT, x0 = (r % tiles_w) * kOT;
         const float* im = img + (size_t)n * 3 * plane;
         __syncthreads();
-        for (int i = threadIdx.x; i < kOP * kOP; i += 256) {
-            const int ty = i / kOP, tx = i - ty * kOP;
-            const int y = y0 + ty - kOR, x = x0 + tx - kOR;
-            tile[ty * (kOP + 1) + tx] = (y >= 0 && y < H && x >= 0 && x < W) ? gray_of(im, plane, (size_t)y * W + x) : 0.f;
-        }
+        orient_stage_gray<0>(im, tile, y0, x0, H, W, plane);
         __syncthreads();
         const int ly = threadIdx.x >> 4, lx = threadIdx.x & 15;
         const int y = y0 + ly, x = x0 + lx;
@@ -68,11 +92,9 @@ __global__ void __launch_bounds__(256) orient_fwd_kernel(const float* __restrict
             }
         }
         if (y < H && x < W) {
-            // resTensor[res < 0] = 0; argmax (first maximum); confidence = (tanh(max) + 1) / 2
-            int best = 0;
-            float mx = fmaxf(acc[0], 0.f);
-#pragma unroll
-            for (int k = 1; k < kOF; ++k) { const float v = fmaxf(acc[k], 0.f); if (v > mx) { mx = v; best = k; } }
+            // confidence = (tanh(max) + 1) / 2
+            float mx;
+            const int best = orient_argmax<0>(acc, mx);
             const size_t pix = (size_t)n * plane + (size_t)y * W + x;
             const float hm = hair[pix];
             const float th = tanhf(mx);
@@ -145,6 +167,83 @@ __global__ void __launch_bounds__(256) orient_bwd_kernel(const float* __restrict
             o[off] = 0.299f * a; o[plane + off] = 0.587f * a; o[2 * plane + off] = 0.144f * a;
         }
     }
+}
+
+// DoG response pass (loss.py:320-340): per pixel r = max_k max(conv_k, 0), idx = its first arg-max, rh = r * hair (fp32
+// product, as the reference's confidenceTensor * mask), and the batch maximum of rh folded into *mbits with an integer atomicMax
+// (rh >= 0, so the order of the bit patterns is the order of the values; the caller zeroes *mbits).
+__global__ void __launch_bounds__(256) dog_response_kernel(const float* __restrict__ img, const float* __restrict__ bank_g,
+                                                           const float* __restrict__ hair, unsigned char* __restrict__ idx_out,
+                                                           float* __restrict__ rh_out, int* __restrict__ mbits, int N, int H, int W) {
+    extern __shared__ float sm[];
+    float* bank = sm;                        // 289 * 32
+    float* tile = sm + kOK * kOK * kOF;      // 32 * 33
+    const int tiles_w = (W + kOT - 1) / kOT, tiles_h = (H + kOT - 1) / kOT;
+    const size_t plane = (size_t)H * W;
+    for (int i = threadIdx.x; i < kOK * kOK * kOF; i += 256) bank[i] = bank_g[i];
+    float m = 0.f;
+    for (int t = blockIdx.x; t < N * tiles_h * tiles_w; t += gridDim.x) {
+        const int n = t / (tiles_h * tiles_w), r = t - n * tiles_h * tiles_w;
+        const int y0 = (r / tiles_w) * kOT, x0 = (r % tiles_w) * kOT;
+        __syncthreads();
+        orient_stage_gray<1>(img + (size_t)n * 3 * plane, tile, y0, x0, H, W, plane);
+        __syncthreads();
+        const int ly = threadIdx.x >> 4, lx = threadIdx.x & 15;
+        const int y = y0 + ly, x = x0 + lx;
+        // the accumulation of orient_fwd_kernel (kept in each kernel: moved into a shared function it changes the Gabor
+        // kernel's register allocation)
+        float acc[kOF];
+#pragma unroll
+        for (int k = 0; k < kOF; ++k) acc[k] = 0.f;
+        for (int i = 0; i < kOK; ++i) {
+#pragma unroll
+            for (int j = 0; j < kOK; ++j) {
+                const float g = tile[(ly + i) * (kOP + 1) + lx + j];
+                const float4* b4 = reinterpret_cast<const float4*>(bank + (i * kOK + j) * kOF);
+#pragma unroll
+                for (int k4 = 0; k4 < kOF / 4; ++k4) {
+                    const float4 b = b4[k4];
+                    acc[4 * k4] = fmaf(g, b.x, acc[4 * k4]); acc[4 * k4 + 1] = fmaf(g, b.y, acc[4 * k4 + 1]);
+                    acc[4 * k4 + 2] = fmaf(g, b.z, acc[4 * k4 + 2]); acc[4 * k4 + 3] = fmaf(g, b.w, acc[4 * k4 + 3]);
+                }
+            }
+        }
+        if (y < H && x < W) {
+            float mx;
+            const int best = orient_argmax<1>(acc, mx);
+            const size_t pix = (size_t)n * plane + (size_t)y * W + x;
+            const float rh = __fmul_rn(mx, hair[pix]);
+            idx_out[pix] = (unsigned char)best;
+            rh_out[pix] = rh;
+            m = fmaxf(m, rh);
+        }
+    }
+    for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(mbits, __float_as_int(m));
+}
+
+// mg_conv_thin with argmax_idx set (see the header): the geometry of the DoG bank is the only one accepted
+int orient_argmax_conv(const mg_thin_args* a, cudaStream_t stream) {
+    if (!a->argmax_mask || !a->argmax_max || !a->out) return set_error(-1, "mg_conv_thin: the arg-max epilogue needs out, argmax_mask and argmax_max");
+    if (a->CinP != 3 || a->Cout != kOF || a->KH != kOK || a->KW != kOK || a->stride != 1 || a->pad != kOR || a->pad_mode != 0 ||
+        a->OH != a->H || a->OW != a->W || a->N < 1 || a->H < 1 || a->W < 1)
+        return set_error(-2, "mg_conv_thin: the arg-max epilogue takes an NCHW RGB image (CinP 3), 32 17x17 filters, stride 1, zero pad 8");
+    if (a->bias || a->pscale || a->pmul || a->out_hi || a->out_lo || a->seg_resize || a->act || a->round_out)
+        return set_error(-3, "mg_conv_thin: the arg-max epilogue has no bias, activation, pixel scales, rounding or 16-bit copies");
+    const size_t smem = (size_t)(kOK * kOK * kOF + kOP * (kOP + 1)) * sizeof(float);
+    static thread_local int attr_dev = -1;
+    int dev = 0; cudaGetDevice(&dev);
+    if (attr_dev != dev) {
+        const cudaError_t e = cudaFuncSetAttribute(dog_response_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+        if (e != cudaSuccess) return set_error((int)e, "orient attr: %s", cudaGetErrorString(e));
+        attr_dev = dev;
+    }
+    const int tiles = a->N * ((a->H + kOT - 1) / kOT) * ((a->W + kOT - 1) / kOT);
+    int grid = 4 * num_sms();
+    if (grid > tiles) grid = tiles;
+    dog_response_kernel<<<grid, 256, smem, stream>>>(a->in, a->w, a->argmax_mask, static_cast<unsigned char*>(a->argmax_idx), a->out,
+                                                     reinterpret_cast<int*>(a->argmax_max), a->N, a->H, a->W);
+    return check_launch("mg_conv_thin");
 }
 
 }  // namespace mg

@@ -6,7 +6,7 @@ without --remove_background), evaluated by the fused reduction kernels of csrc/m
     fp64 accumulation) and ONE backward launch, instead of ~10 eager ops per scale and per term;
   * the wide-edge weight map (loss.py:60-78) is one kernel per scale, cached per (label, size) within an iteration.
 
-The rest of the generator objective follows: the Gabor orientation loss, VGGLoss / StyleContentLoss (every VGG19 term from one
+The rest of the generator objective follows: the Gabor and DoG orientation losses, VGGLoss / StyleContentLoss (every VGG19 term from one
 pass, _VGGObjectiveFn), LabColorLoss and HairAvgLabLoss (with or without --balance_Lab), RGBBackgroundL1Loss and the rgb L1
 (RGBL1Loss).
 """
@@ -32,7 +32,9 @@ class _Term(C.Structure):
                 # appended for the accumulating backward (null: ga is written, not accumulated)
                 ("add", C.c_void_p),
                 # appended for op 11 (null for every other op)
-                ("table", C.c_void_p)]
+                ("table", C.c_void_p),
+                # appended for op 12 (null for every other op)
+                ("idx", C.c_void_p), ("maxv", C.c_void_p)]
 
 
 OP_HINGE_D, OP_SUM, OP_L1, OP_SQ = 0, 1, 2, 3
@@ -42,6 +44,8 @@ OP_BCE, OP_SQ_T, OP_WSUM, OP_HINGE_MASK, OP_L1_MASK = 4, 5, 6, 7, 8
 OP_SQ_MASK, OP_MOMENTS = 9, 10
 # LabColorLoss with --balance_Lab: the Lab L1 weighted per pixel by the count table of the real pixel's (a, b) bins
 OP_LAB_BALANCED = 11
+# L1OLoss with the DoG filter: both losses of the batch-normalised confidence and the sums of the gradient through its maximum
+OP_ORIENT_DOG = 12
 MASKED_OPS = (OP_WSUM, OP_HINGE_MASK, OP_L1_MASK, OP_SQ_MASK)      # one scalar term over its own sum(label1) * c + 1e-5
 DEN_EPS = 1e-5          # loss.py:111, 114, 117, 160, 196, 677: sum(label1) * c + 1e-5
 _table_cache = {}
@@ -339,6 +343,95 @@ class _OrientLossFn(torch.autograd.Function):
         _lib.check(_lib.load().mg_orient_loss_bwd(bank.data_ptr(), idx.data_ptr(), d1.data_ptr(), d2.data_ptr(), wts.data_ptr(), dimg.data_ptr(),
                                                   n, h, w, ops._stream()), "mg_orient_loss_bwd")
         return dimg, None, None, None
+
+
+# ================================================================================================ DoG orientation loss
+def dog_bank(device, num_kernels=32, kernel_size=17):
+    """The 32 Difference-of-Gaussians kernels the reference rebuilds on every call (DoG_fn, loss.py:245-271; sigma_h 1,
+    sigma_l 2, sigma_y 2, theta_k = pi*k/32), with the same float32 torch operations (one 17x17 kernel at a time, the sigmas as
+    device tensors), laid out [17*17][32] like gabor_bank."""
+    import math
+    r = kernel_size // 2
+    y = torch.arange(-r, r + 1, device=device).view(1, -1).repeat(kernel_size, 1).float()       # varies along columns
+    x = torch.arange(-r, r + 1, device=device).view(-1, 1).repeat(1, kernel_size).float()       # varies along rows
+    s_h, s_l, s_y = (torch.ones(1, device=device) * v for v in (1.0, 2.0, 2.0))
+    ks = []
+    for k in range(num_kernels):
+        theta = torch.ones(1, device=device) * (math.pi * k / num_kernels)
+        x_t = x * torch.cos(theta) + y * torch.sin(theta)
+        y_t = -x * torch.sin(theta) + y * torch.cos(theta)
+        hi = torch.exp(-.5 * (x_t ** 2 / s_h ** 2 + y_t ** 2 / s_y ** 2)) / s_h
+        lo = torch.exp(-.5 * (x_t ** 2 / s_l ** 2 + y_t ** 2 / s_y ** 2)) / s_l
+        ks.append((hi - lo) / (1.0 / s_h - 1.0 / s_l))
+    return torch.stack(ks, dim=-1).reshape(kernel_size * kernel_size, num_kernels).contiguous()
+
+
+def _orient_sincos(device, num_kernels=32):
+    """[2][32]: sin and cos of 2 * (k * pi / 32), the angle of filter k as the reference forms it from the arg-max
+    (loss.py:345-348), in fp32 torch arithmetic on the device."""
+    import math
+    a = torch.arange(num_kernels, device=device).float() * math.pi / num_kernels
+    return torch.stack([torch.sin(2 * a), torch.cos(2 * a)]).contiguous()
+
+
+def _pinned_table(term, device):
+    """One _Term record -> device bytes, through pinned memory and an asynchronous copy (no host synchronisation; the
+    caching host allocator keeps the pinned block until the copy has run)."""
+    raw = torch.frombuffer(bytearray(bytes(term)), dtype=torch.uint8)
+    if device.type != "cuda":           # tests/dryrun.py runs the glue on the CPU
+        return raw
+    return raw.pin_memory().to(device, non_blocking=True)
+
+
+class _DoGOrientLossFn(torch.autograd.Function):
+    """L1OLoss with the DoG filter (loss.py:320-385) in three launches forward (response pass, mg_loss_reduce op 12) and two
+    backward (mg_loss_reduce_bwd op 12 -> dL/dr, then the orientation loss's bank-generic gather).  M, the sums and the tie
+    count stay on the device."""
+
+    @staticmethod
+    def forward(ctx, img, bank, sincos, label2, hair):
+        n, _, h, w = img.shape
+        dev = img.device
+        if n * h * w >= 2 ** 31:
+            raise ValueError("L1OLoss (DoG): at most 2^31 - 1 pixels per call, got %d" % (n * h * w))
+        idx, rh, m = ops.dog_response(img.detach().contiguous(), bank, hair)
+        slots = torch.zeros(6, device=dev, dtype=torch.float64)
+        term = _dog_term(rh, label2, hair, idx, m, sincos, None)
+        table = _pinned_table(term, dev)
+        _lib.check(_lib.load().mg_loss_reduce(table.data_ptr(), 1, slots.data_ptr(), ops._stream()), "mg_loss_reduce")
+        ctx.save_for_backward(bank, sincos, label2, hair, idx, rh, m, slots)
+        ctx.keep = table
+        orient = (slots[0] / (2.0 * n * h * w)).float().reshape(())
+        conf = (slots[1] / (slots[2] + DEN_EPS)).float().reshape(())
+        return orient, conf
+
+    @staticmethod
+    def backward(ctx, g_orient, g_conf):
+        bank, sincos, label2, hair, idx, rh, m, slots = ctx.saved_tensors
+        n, h, w = rh.shape
+        dev = rh.device
+        go = g_orient.double().reshape(()) / (2.0 * n * h * w)
+        gc = g_conf.double().reshape(()) / (slots[2] + DEN_EPS)
+        # the gradient through M, split evenly among the pixels that attain it (torch's rule for max())
+        share = (go * slots[3] + gc * slots[4]) / slots[5]
+        gslots = torch.stack([go, gc, share]).float().contiguous()
+        dr = torch.empty((n, h, w), device=dev, dtype=torch.float32)
+        table = _pinned_table(_dog_term(rh, label2, hair, idx, m, sincos, dr.data_ptr()), dev)
+        _lib.check(_lib.load().mg_loss_reduce_bwd(table.data_ptr(), 1, gslots.data_ptr(), ops._stream()), "mg_loss_reduce_bwd")
+        wts = torch.cat([torch.ones(1, device=dev), torch.zeros(1, device=dev)])     # the gather's weights: dr alone
+        dimg = torch.empty((n, 3, h, w), device=dev, dtype=torch.float32)
+        _lib.check(_lib.load().mg_orient_loss_bwd(bank.data_ptr(), idx.data_ptr(), dr.data_ptr(), dr.data_ptr(), wts.data_ptr(),
+                                                  dimg.data_ptr(), n, h, w, ops._stream()), "mg_orient_loss_bwd")
+        return dimg, None, None, None, None
+
+
+def _dog_term(rh, label2, hair, idx, m, sincos, ga):
+    """The op 12 record: a = rh, b = label2 [N,2,H,W], label = hair [N,H,W], idx, maxv = M, table = the (sin, cos) table."""
+    n, h, w = rh.shape
+    t = _Term(rh.data_ptr(), label2.data_ptr(), ga, n * h * w, 1.0, 1.0, OP_ORIENT_DOG, 0)
+    t.label, t.label_ns, t.h, t.w, t.H, t.W = hair.data_ptr(), h * w, h, w, h, w
+    t.table, t.idx, t.maxv = sincos.data_ptr(), idx.data_ptr(), m.data_ptr()
+    return t
 
 
 VGG_WEIGHTS = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
@@ -880,25 +973,34 @@ class HairAvgLabLoss(nn.Module):
 
 
 class L1OLoss(nn.Module):
-    """loss.py:274-385 with orient_filter='gabor': (orient_loss, confidence_loss) = forward(fake_image, orientation_label,
-    input_semantics).  orientation_label: the 1-channel angle map (0..255) or, with --use_ig, the 2-channel (sin 2t, cos 2t) map."""
+    """loss.py:274-385: (orient_loss, confidence_loss) = forward(fake_image, orientation_label, input_semantics).
+    orientation_label: the 1-channel angle map (0..255) or, with --use_ig, the 2-channel (sin 2t, cos 2t) map.
+
+    orient_filter containing 'gabor' selects the Gabor bank (confidence (tanh(r) + 1) / 2, log confidence loss); any other value
+    the Difference-of-Gaussians bank, whose confidence r * hair / M is normalised by M, the maximum over the batch of this call,
+    with the L1 confidence loss against the hair mask.  Under data parallelism M is taken over each rank's shard, as each of the
+    reference's DataParallel replicas took it over its own; it is not reduced across ranks.  A batch without hair has M = 0 and
+    both losses and the gradient are NaN, as in the reference."""
 
     def __init__(self, opt, channel_in=1, channel_out=1, stride=1, padding=8):
         super().__init__()
-        if "gabor" not in getattr(opt, "orient_filter", "gabor"):
-            raise NotImplementedError("michigan_b200: orient_filter '%s' (the DoG variant has no kernel)" % opt.orient_filter)
         self.opt = opt
+        self.dog = "gabor" not in getattr(opt, "orient_filter", "gabor")
         self._bank = None
+        self._sincos = None
 
     def forward(self, fake_image0, orientation_label0, input_semantics):
         import math
         dev = fake_image0.device
         if self._bank is None or self._bank.device != dev:
-            self._bank = gabor_bank(dev)
+            self._bank = dog_bank(dev) if self.dog else gabor_bank(dev)
+            self._sincos = _orient_sincos(dev) if self.dog else None
         hair = input_semantics[:, 1].contiguous().float()
         if not self.opt.use_ig:
             t = orientation_label0.float() / 255 * math.pi
             label2 = torch.cat([torch.sin(2 * t), torch.cos(2 * t)], dim=1).contiguous()
         else:
             label2 = orientation_label0.float().contiguous()
+        if self.dog:
+            return _DoGOrientLossFn.apply(fake_image0, self._bank, self._sincos, label2.detach(), hair.detach())
         return _OrientLossFn.apply(fake_image0, self._bank, label2.detach(), hair.detach())

@@ -205,6 +205,25 @@ def conv_thin(x, wt, bias, cout, kh, kw, stride=1, pad=0, *, pad_mode=0, seg_res
     return out
 
 
+def dog_response(img_nchw, bank, hair):
+    """The DoG orientation response pass of L1OLoss (mg_conv_thin's arg-max epilogue): img [N,3,H,W] in [-1,1], bank the
+    [17*17][32] filters, hair [N,H,W] -> (idx [N,H,W] uint8 first arg-max of the clamped responses, rh [N,H,W] = max response *
+    hair, m [1] = max of rh over the batch, on the device)."""
+    _chk(img_nchw, "img"); _chk(bank, "bank"); _chk(hair, "hair")
+    N, _, H, W = img_nchw.shape
+    idx = torch.empty((N, H, W), device=img_nchw.device, dtype=torch.uint8)
+    rh = torch.empty((N, H, W), device=img_nchw.device, dtype=torch.float32)
+    m = torch.zeros(1, device=img_nchw.device, dtype=torch.float32)
+    a = ThinArgs()
+    a.inp, a.w, a.out = _p(img_nchw), _p(bank), _p(rh)
+    a.N, a.H, a.W, a.CinP = N, H, W, 3
+    a.OH, a.OW, a.Cout = H, W, 32
+    a.KH, a.KW, a.stride, a.pad = 17, 17, 1, 8
+    a.argmax_idx, a.argmax_mask, a.argmax_max = _p(idx), _p(hair), _p(m)
+    check(_lib.load().mg_conv_thin(C.byref(a), _stream()), "mg_conv_thin")
+    return idx, rh, m
+
+
 def pack_weight_seg_tc(w_oihw):
     """bf16 [128][128] operand of conv_seg_tc: k = part*36 + tap*4 + ci with parts (W_hi, W_hi, W_lo)."""
     _chk(w_oihw, "w")
