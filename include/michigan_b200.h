@@ -374,6 +374,8 @@ int mg_edge_weight(const float* label, float* out, int N, int H, int W, int h, i
  *          Backward: gslots[out_slot + 0..2] = (go, gc, share), share = (go slot3 + gc slot4) / slot5 formed by the caller;
  *          ga = dL/dr = hair ((go Lo + gc Lc) / M + [rh == M] share) (add is not applied).  idx and maxv are null for every
  *          other op.
+ *   op 13: f = e^a - a - 1 (expm1f(a) - a)         the logvar half of KLDLoss, loss.py:211-213: -0.5 sum(1 + logvar -
+ *          mu^2 - e^logvar) = 0.5 sum mu^2 (op 3 with b = 0) + 0.5 sum (e^logvar - logvar - 1); df/da = e^a - 1 (expm1f(a)).
  * mg_loss_reduce_bwd writes ga_i = add_i + gslots[out_slot] * scale * df/da for every term with ga != null (add null: ga_i =
  * gslots[out_slot] * scale * df/da; add may alias ga; no two terms of one launch may write the same ga).  Torch's tie rules:
  * the binary min gives each side half, |.| has gradient 0 at 0; BCE: sigmoid(a) - target.  Op 9: df/da = 2 (a l - b l) l.

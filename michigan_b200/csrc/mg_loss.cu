@@ -142,7 +142,7 @@ __device__ __forceinline__ int term_channel(const LossTerm& t, long long i) {
     return (int)(t.channels_last ? i % t.C : (i / ((long long)t.h * t.w)) % t.C);
 }
 
-// f of ops 4-9 at element i (l = the element's label for ops 6-9)
+// f of ops 4-9 and 13 at element i (l = the element's label for ops 6-9)
 __device__ __forceinline__ float term_f(const LossTerm& t, float a, long long i, float l) {
     switch (t.op) {
     case 4: return __fmul_rn(1.f - t.target, a) + fmaxf(-a, 0.f) + log1pf(expf(-fabsf(a)));
@@ -150,11 +150,12 @@ __device__ __forceinline__ float term_f(const LossTerm& t, float a, long long i,
     case 6: return __fmul_rn(a, l);
     case 7: return fminf(__fmul_rn(t.sign * a - 1.f, l), 0.f);
     case 9: return sq_diff(__fmul_rn(a, l), __fmul_rn(__ldg(t.b + i), l));
+    case 13: return expm1f(a) - a;
     default: return fabsf(__fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l));
     }
 }
 
-// df/da of ops 4-10; ties as torch: the binary min gives each side half, |.| has gradient 0 at 0
+// df/da of ops 4-10 and 13; ties as torch: the binary min gives each side half, |.| has gradient 0 at 0
 __device__ __forceinline__ float term_df(const LossTerm& t, float a, long long i, float l) {
     switch (t.op) {
     case 4: {
@@ -169,6 +170,7 @@ __device__ __forceinline__ float term_df(const LossTerm& t, float a, long long i
         return m < 0.f ? t.sign * l : (m == 0.f ? 0.5f * t.sign * l : 0.f);
     }
     case 9: return 2.f * (__fmul_rn(a, l) - __fmul_rn(__ldg(t.b + i), l)) * l;
+    case 13: return expm1f(a);
     case 10: {
         const int n = (int)(i / ((long long)t.C * t.h * t.w)), c = term_channel(t, i);
         const float* co = t.b + (size_t)n * 3 * t.C + c;
@@ -360,8 +362,8 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
         return;
     }
     if (t.op >= 4) {
-        // ops 4-9: one element per thread per trip, fp32 partials per thread, fp64 across threads
-        const bool masked = t.op >= 6;
+        // ops 4-9 and 13: one element per thread per trip, fp32 partials per thread, fp64 across threads
+        const bool masked = t.op >= 6 && t.op <= 9;
         const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;
         float accl = 0.f;
         for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
@@ -401,7 +403,7 @@ __global__ void __launch_bounds__(256) loss_reduce_kernel(const LossTerm* __rest
 }
 
 // ga_i = gslot[out_slot] * scale * f'(a_i):  op 0: sign * w_i * ([sign*a - 1 < 0] + [sign*a - 1 == 0] / 2);  op 1: 1;
-// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10: term_df;  op 11: balanced_lab_term_bwd;  op 12: dog_orient_term_bwd.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
+// op 2: sgn(a - b);  op 3: 2 (a - b);  ops 4-10, 13: term_df;  op 11: balanced_lab_term_bwd;  op 12: dog_orient_term_bwd.  Op 0 at a tie: torch's binary min (the reference's torch.min(x - 1, 0))
 // gives each side half the gradient.  The masked ops' denominators are folded into gslot by the caller.  With t.add the
 // result is added to add_i (which may be ga itself: each element is read before the same thread writes it).
 __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __restrict__ terms, const float* __restrict__ gslots) {
@@ -417,7 +419,7 @@ __global__ void __launch_bounds__(256) loss_reduce_bwd_kernel(const LossTerm* __
         return;
     }
     if (t.op >= 4) {
-        const bool masked = t.op >= 6;
+        const bool masked = t.op >= 6 && t.op <= 10;
         const float sh = masked ? (float)t.H / (float)t.h : 0.f, sw = masked ? (float)t.W / (float)t.w : 0.f;
         for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < t.n; i += (long long)gridDim.x * blockDim.x) {
             const float l = masked ? term_label(t, i, sh, sw) : 0.f;

@@ -55,6 +55,8 @@ def install(reference_root=None, compat=True):
     arc.SPADE = mine.SPADE
     enc.ImageEncoder3 = mine.ImageEncoder3
     enc.BackgroundEncode2 = mine.BackgroundEncode2
+    # --use_vae: define_E finds 'convencoder' in models.networks.encoder (networks/__init__.py:65-68)
+    enc.ConvEncoder = both(mine.ConvEncoder)
     for name in ("SynchronizedBatchNorm1d", "SynchronizedBatchNorm2d", "SynchronizedBatchNorm3d", "DataParallelWithCallback",
                  "patch_replication_callback", "convert_model", "patch_sync_batchnorm"):
         setattr(sbn, name, getattr(mine.sync_batchnorm, name))
@@ -62,10 +64,12 @@ def install(reference_root=None, compat=True):
     # the GAN and GAN feature-matching losses (pix2pix_model.py:36-39, networks.GANLoss, networks.GANFeatLoss), the perceptual,
     # style / content, background and Lab colour losses (pix2pix_model.py:41-53 look them up as networks.VGGLoss,
     # networks.StyleContentLoss, networks.RGBBackgroundL1Loss, networks.LabColorLoss) and the hair-average Lab loss of the
-    # unpaired stage (pix2pix_model.py:55-56, networks.HairAvgLabLoss).  The rgb term is a bare nn.L1Loss (pix2pix_model.py:51)
+    # unpaired stage (pix2pix_model.py:55-56, networks.HairAvgLabLoss), and the KL divergence of --use_vae (pix2pix_model.py:42-43,
+    # networks.KLDLoss).  The rgb term is a bare nn.L1Loss (pix2pix_model.py:51)
     # and stays torch's: torch.nn is not patched.
     los = importlib.import_module("models.networks.loss")
-    for name in ("GANLoss", "GANFeatLoss", "VGGLoss", "StyleContentLoss", "RGBBackgroundL1Loss", "LabColorLoss", "HairAvgLabLoss"):
+    for name in ("GANLoss", "GANFeatLoss", "VGGLoss", "StyleContentLoss", "RGBBackgroundL1Loss", "LabColorLoss", "HairAvgLabLoss",
+                 "KLDLoss"):
         setattr(los, name, getattr(mine.loss, name))
         setattr(pkg, name, getattr(mine.loss, name))
     if getattr(gen, "InpaintGenerator", None) is not None:

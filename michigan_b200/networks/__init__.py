@@ -7,8 +7,8 @@ from .base_network import BaseNetwork
 from .normalization import SPADE, get_nonspade_norm_layer
 from .architecture import SPADEResnetBlock, VGG19
 from . import loss
-from .loss import GANLoss, GANFeatLoss, VGGLoss, LabColorLoss, StyleContentLoss, RGBBackgroundL1Loss, HairAvgLabLoss
-from .encoder import ImageEncoder3, BackgroundEncode2, PartialConv2d, ConvBlock
+from .loss import GANLoss, GANFeatLoss, VGGLoss, LabColorLoss, StyleContentLoss, RGBBackgroundL1Loss, HairAvgLabLoss, KLDLoss
+from .encoder import ImageEncoder3, BackgroundEncode2, PartialConv2d, ConvBlock, ConvEncoder
 from .generator import SPADEBGenerator
 from .discriminator import MultiscaleDiscriminator, NLayerDiscriminator
 from .inpaint import InpaintGenerator
@@ -17,11 +17,12 @@ from .sync_batchnorm import SynchronizedBatchNorm2d, DataParallelWithCallback
 
 _GENERATORS = {"spadeb": SPADEBGenerator, "inpaint": InpaintGenerator}
 _DISCRIMINATORS = {"multiscale": MultiscaleDiscriminator, "nlayer": NLayerDiscriminator, "n_layer": NLayerDiscriminator}
+_ENCODERS = {"conv": ConvEncoder}
 
 
 def find_network_using_name(target_network_name, filename):
     """networks/__init__.py:16-24: `<name><filename>` looked up case-insensitively."""
-    table = {"generator": _GENERATORS, "discriminator": _DISCRIMINATORS}.get(filename)
+    table = {"generator": _GENERATORS, "discriminator": _DISCRIMINATORS, "encoder": _ENCODERS}.get(filename)
     if table is None or target_network_name.lower() not in table:
         raise ValueError("In %s.py, there should be a class name that matches %s in lowercase (michigan_b200 "
                          "implements netG=spadeb, netD=multiscale)" % (filename, target_network_name + filename))
@@ -58,3 +59,8 @@ def define_IG(opt):
 
 def define_D(opt):
     return create_network(find_network_using_name(opt.netD, "discriminator"), opt)
+
+
+def define_E(opt):
+    """networks/__init__.py:65-68: the --use_vae image encoder (there is one encoder type, 'conv')."""
+    return create_network(find_network_using_name("conv", "encoder"), opt)

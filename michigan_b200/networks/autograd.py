@@ -1,5 +1,5 @@
-"""Training path: hand-written backward passes wired into torch.autograd as two Functions
-(generator, multiscale discriminator).  Forward = the networks' ONE forward implementation (`SPADEBGenerator.run`,
+"""Training path: hand-written backward passes wired into torch.autograd as three Functions
+(generator, multiscale discriminator, the --use_vae ConvEncoder).  Forward = the networks' ONE forward implementation (`SPADEBGenerator.run`,
 `MultiscaleDiscriminator.run`) in "save" mode: the same kernels and operand formats as inference (precision.py), which
 additionally keep the fp32 value of every tensor the gradient GEMMs need (read as TF32 by the wgrad / dgrad kernels);
 backward = explicit reverse pass over the saved per-block state:
@@ -181,12 +181,30 @@ def bg_bwd(G, bg, S, dfeats):
     G.add(bg.conv1.conv.weight, _thin_wt_to_oihw(dwt1, 7, 7, 3))
 
 
+def latent_bwd(G, fc, S, dx):
+    """Backward of the --use_vae latent head x = view(z W^T + b) (generator.py:110-116) given dx [N,sh,sw,16nf] NHWC;
+    returns dz [N, z_dim].  The weight and bias gradients read dx in the reference's NCHW row order (one transpose of the
+    N x 16nf*sh*sw gradient), so they come out in fc.weight's own layout.  They are one weight-gradient GEMM over the N rows:
+    z is extended by a column of ones (the bias) and 31 zeros (the GEMM's 32-column granule), so dW | db = dY^T [z | 1 | 0]
+    (the per-channel sum kernels take at most 4096 channels; the head has 16nf*sh*sw).  dz is the 1x1 data-gradient GEMM on
+    the permuted weight the forward packed (S.wp)."""
+    N = dx.shape[0]
+    K = dx[0].numel()
+    dy_ref = ops.nhwc_to_nchw(dx).view(N, 1, 1, K)
+    zd = S.z4.shape[-1]
+    za = torch.cat([S.z4.view(N, zd), torch.ones((N, 1), device=dx.device), torch.zeros((N, 31), device=dx.device)], 1)
+    dwa = ops.conv_wgrad(dy_ref, za.view(N, 1, 1, zd + 32), 1, 1, 1, 0)
+    G.add(fc.weight, dwa[:, :zd])
+    G.add(fc.bias, dwa[:, zd])
+    return ops.conv_dgrad(dx.view(N, 1, 1, K), S.wp.view(K, -1, 1, 1), (1, 1), 1, 0).view(N, -1)
+
+
 # =============================================================================================== generator Function
 class _GeneratorFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, netG, input_ref, orient_mask, image_ref, input_tag, noise, image_tag, *params):
+    def forward(ctx, netG, z, input_ref, orient_mask, image_ref, input_tag, noise, image_tag, *params):
         st = SimpleNamespace()
-        out = netG.run(input_ref, orient_mask, image_ref, input_tag, noise, image_tag, st)
+        out = netG.run(input_ref, orient_mask, image_ref, input_tag, noise, image_tag, st, z=z)
         ctx.netG, ctx.seg4, ctx.inv_of, ctx.saved, ctx.Sfc, ctx.Sbg, ctx.x_last, ctx.out = \
             netG, st.seg4, st.inv_of, st.saved, st.Sfc, st.Sbg, st.x_last, st.out
         ctx.params = params
@@ -213,18 +231,81 @@ class _GeneratorFn(torch.autograd.Function):
                 dfeats[idx - 3] = dbf
             if red is not None and names[idx] in stage_of:
                 red.reduce_stage(stage_of[names[idx]], G.get)
-        fc_bwd(G, netG.fc, ctx.Sfc, dx)
+        dz = None
+        if getattr(netG.opt, "use_vae", False):
+            dz = latent_bwd(G, netG.fc, ctx.Sfc, dx)
+            if not ctx.needs_input_grad[1]:
+                dz = None
+        else:
+            fc_bwd(G, netG.fc, ctx.Sfc, dx)
         bg_bwd(G, netG.backgroud_enc, ctx.Sbg, dfeats)
         ctx.saved = ctx.Sfc = ctx.Sbg = None
         if red is not None:
             red.reduce_stage(len(red.stages) - 1, G.get)
-            return (None,) * 7 + red.finish(ctx.params, G.get)
-        return (None,) * 7 + tuple(G.get(p) for p in ctx.params)
+            return (None, dz) + (None,) * 6 + red.finish(ctx.params, G.get)
+        return (None, dz) + (None,) * 6 + tuple(G.get(p) for p in ctx.params)
 
 
-def generator_forward_autograd(netG, input_ref, orient_mask, image_ref, input_tag, noise, image_tag):
+def generator_forward_autograd(netG, input_ref, orient_mask, image_ref, input_tag, noise, image_tag, z=None):
     params = [p for p in netG.parameters()]
-    return _GeneratorFn.apply(netG, input_ref, orient_mask, image_ref, input_tag, noise, image_tag, *params)
+    return _GeneratorFn.apply(netG, z, input_ref, orient_mask, image_ref, input_tag, noise, image_tag, *params)
+
+
+# =============================================================================================== ConvEncoder Function
+def conv_encoder_bwd(G, E, S, dout):
+    """Parameter gradients of ConvEncoder.run given dout = d(mu | logvar) [N,1,1,512]: fc_mu | fc_var weight and bias, then the
+    six SN conv + InstanceNorm + LeakyReLU layers in reverse, as _d_scale_bwd does for the discriminator's convs."""
+    N = dout.shape[0]
+    dwf = ops.conv_wgrad(dout, S.a6, 1, 1, 1, 0)                  # [512, 16C], columns in the map's NHWC order
+    c = S.y6.shape[-1]
+    dwf = dwf.view(512, 16, c).transpose(1, 2).reshape(512, 16 * c)
+    G.add(E.fc_mu.weight, dwf[:256])
+    G.add(E.fc_var.weight, dwf[256:])
+    db = ops.chan_sum(dout)
+    G.add(E.fc_mu.bias, db[:256])
+    G.add(E.fc_var.bias, db[256:])
+    da = ops.conv_dgrad(dout, E.fc_weight(), (1, 1), 1, 0).view(S.y6.shape)
+    dy = ops.in_bwd(da, S.y6, S.ss6, _LRELU, round_tf32=True)
+    for L in reversed(S.layers):
+        _conv_param_grads(G, L.conv, S.inv_of, dy, L.a, 3, 3, 2, 1, with_bias=False)
+        w, isg, _ = _conv_weight(L.conv, S.inv_of)
+        da = ops.conv_dgrad(dy, w.detach(), (L.a.shape[1], L.a.shape[2]), 2, 1, inv_sigma=isg)
+        dy = ops.in_bwd(da, L.y_in, L.ss, _LRELU, round_tf32=L is not S.layers[0])
+    conv1 = E.layer1[0]
+    w1, isg1, is_sn = _conv_weight(conv1, S.inv_of)
+    dwt = _thin_wt_to_oihw(ops.thin_wgrad(S.x0, dy, 3, 3, 2, 1), 3, 3, 3)
+    G.add(w1, ops.spectral_norm_bwd(dwt, w1.detach(), conv1.weight_u, conv1.weight_v, isg1) if is_sn else dwt)
+
+
+class _ConvEncoderFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, netE, image, *params):
+        st = SimpleNamespace()
+        mu, logvar = netE.run(image, st)
+        ctx.netE, ctx.st, ctx.params = netE, st, params
+        return mu, logvar
+
+    @staticmethod
+    def backward(ctx, dmu, dlogvar):
+        netE = ctx.netE
+        G = _Grads()
+        red = getattr(netE, "_grad_reducer", None)
+        if red is not None:
+            red.begin(ctx.params)
+        N = ctx.st.y6.shape[0]
+        dmu = torch.zeros((N, 256), device=ctx.st.y6.device) if dmu is None else dmu
+        dlogvar = torch.zeros((N, 256), device=ctx.st.y6.device) if dlogvar is None else dlogvar
+        dout = torch.cat([dmu, dlogvar], dim=1).float().view(N, 1, 1, 512)
+        conv_encoder_bwd(G, netE, ctx.st, dout)
+        ctx.st = None
+        if red is not None:
+            red.reduce_stage(0, G.get)
+            return (None, None) + red.finish(ctx.params, G.get)
+        return (None, None) + tuple(G.get(p) for p in ctx.params)
+
+
+def conv_encoder_forward_autograd(netE, image):
+    return _ConvEncoderFn.apply(netE, image, *netE.parameters())
 
 
 # =============================================================================================== discriminator Function

@@ -1,7 +1,7 @@
 """Sub-networks instantiated inside SPADEBGenerator: the partial-conv reference encoder
 (reference models/networks/encoder.py:160-225, partialconv2d.py:15-85) and the background encoder
-(encoder.py:271-341, MaskGAN_networks.py:114-173).  Same constructors and state-dict keys; forward on
-the CUDA kernels, NHWC inside."""
+(encoder.py:271-341, MaskGAN_networks.py:114-173); and the --use_vae image encoder `ConvEncoder` (encoder.py:17-59, the
+reference's netE).  Same constructors and state-dict keys; forward on the CUDA kernels, NHWC inside."""
 import random
 from types import SimpleNamespace
 
@@ -11,7 +11,8 @@ import torch.nn as nn
 
 from .. import ops, precision
 from .base_network import BaseNetwork
-from .prep import PackCache
+from .normalization import get_nonspade_norm_layer
+from .prep import PackCache, SpectralNormBatch
 
 
 class PartialConv2d(nn.Conv2d):
@@ -199,3 +200,130 @@ class BackgroundEncode2(BaseNetwork):
         sh, sw = bm.shape[2:]
         masks = [F.interpolate(bm, size=(int(sh / d), int(sw / d)), mode="nearest") for d in (8, 4, 2)] + [bm]
         return [f.permute(0, 3, 1, 2) for f in feats], masks
+
+
+class ConvEncoder(BaseNetwork):
+    """encoder.py:17-59, the --use_vae encoder: image -> (mu, logvar), each [N, 256].
+
+    The image is resized to 256x256 (bilinear, align_corners=False), then six k3 s2 p1 convs, each normalised by
+    `norm_E` (spectral norm, bias removed, InstanceNorm2d without affine) and followed by LeakyReLU 0.2, give a
+    [N, 8ngf, 4, 4] map; fc_mu and fc_var read it flattened in NCHW order.  On the kernels: layer1 is the thin direct conv,
+    layers 2-6 the implicit-GEMM conv under the precision.conv_fmt policy, and fc_mu | fc_var one 1x1 implicit GEMM whose
+    rows are the images, with the two weights concatenated and their columns permuted once into the NHWC order of the
+    map (cached until the weights change).  Training runs one in-place power iteration per forward, as torch's
+    spectral_norm does; eval uses the stored u, v.  The backward is autograd.conv_encoder_bwd; the image gets no gradient
+    (the reference encodes image_ref.clone() of a tensor that needs none)."""
+
+    def __init__(self, opt):
+        super().__init__()
+        if opt.crop_size < 256:
+            raise NotImplementedError("michigan_b200: --use_vae needs crop_size >= 256: below it the reference's ConvEncoder "
+                                      "has no layer6 and fc_mu does not match its 8x8 map")
+        if opt.z_dim != 256:
+            raise NotImplementedError("michigan_b200: --use_vae needs z_dim 256: the reference's fc_mu / fc_var have 256 "
+                                      "outputs whatever z_dim says")
+        if opt.norm_E not in ("spectralinstance", "instance"):
+            raise NotImplementedError("michigan_b200: norm_E '%s' has no CUDA kernel (supported: [spectral]instance)" % opt.norm_E)
+        if opt.ngf % 32 != 0:
+            raise NotImplementedError("michigan_b200: ngf must be a multiple of 32")
+        kw = 3
+        pw = int(np.ceil((kw - 1.0) / 2))
+        ndf = opt.ngf
+        norm_layer = get_nonspade_norm_layer(opt, opt.norm_E)
+        self.layer1 = norm_layer(nn.Conv2d(3, ndf, kw, stride=2, padding=pw))
+        self.layer2 = norm_layer(nn.Conv2d(ndf * 1, ndf * 2, kw, stride=2, padding=pw))
+        self.layer3 = norm_layer(nn.Conv2d(ndf * 2, ndf * 4, kw, stride=2, padding=pw))
+        self.layer4 = norm_layer(nn.Conv2d(ndf * 4, ndf * 8, kw, stride=2, padding=pw))
+        self.layer5 = norm_layer(nn.Conv2d(ndf * 8, ndf * 8, kw, stride=2, padding=pw))
+        self.layer6 = norm_layer(nn.Conv2d(ndf * 8, ndf * 8, kw, stride=2, padding=pw))
+        self.so = s0 = 4
+        self.fc_mu = nn.Linear(ndf * 8 * s0 * s0, 256)
+        self.fc_var = nn.Linear(ndf * 8 * s0 * s0, 256)
+        self.actvn = nn.LeakyReLU(0.2, False)
+        self.opt = opt
+        self._snb = None
+        self._cache = PackCache()
+
+    def convs(self):
+        return [getattr(self, "layer%d" % i)[0] for i in range(1, 7)]
+
+    def grad_stages(self):
+        """One gradient all-reduce stage: the whole encoder is finished together (autograd.conv_encoder_bwd)."""
+        return [list(self.parameters())]
+
+    def spectral_batch(self):
+        if self._snb is None:
+            self._snb = SpectralNormBatch([c for c in self.convs() if hasattr(c, "weight_orig")])
+        return self._snb
+
+    def fc_weight(self):
+        """[512, 16C, 1, 1] fp32: fc_mu | fc_var with the columns in the NHWC order (h, w, c) of the 4x4 map."""
+        def build():
+            c = self.fc_mu.in_features // 16
+            w = torch.cat([self.fc_mu.weight.detach(), self.fc_var.weight.detach()])
+            return w.view(512, c, 16).transpose(1, 2).reshape(512, 16 * c, 1, 1).contiguous()
+        return self._cache.get("fc_w", [self.fc_mu.weight, self.fc_var.weight], build)
+
+    def forward(self, x):
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            from .autograd import conv_encoder_forward_autograd
+            return conv_encoder_forward_autograd(self, x)
+        return self.run(x, None)
+
+    def run(self, image, save):
+        """The one forward implementation: image [N,3,H,W] NCHW -> (mu, logvar).  save: namespace filled with what
+        autograd.conv_encoder_bwd needs (same arithmetic either way)."""
+        N, _, H, W = image.shape
+        x = ops.nchw_to_nhwc(image.detach().contiguous(), 4)
+        if (H, W) != (256, 256):
+            x = ops.resize_bilinear(x, 256, 256)                               # encoder.py:42-43
+        snb = self.spectral_batch()
+        inv = snb.run(self.training)
+        inv_of = {cv: (inv[i:i + 1].clone() if save is not None else inv[i:i + 1]) for i, cv in enumerate(snb.convs)}
+
+        def weight(conv):
+            return (conv.weight_orig, inv_of[conv]) if hasattr(conv, "weight_orig") else (conv.weight, None)
+
+        conv1 = self.layer1[0]
+        w1, isg1 = weight(conv1)
+        # W / sigma of an 864-element weight, scaled on the device before packing (the thin conv has no sigma input)
+        wt1 = ops.pack_weight_thin(w1.detach() * isg1 if isg1 is not None else w1.detach(), 4)
+        y = ops.conv_thin(x, wt1, None, conv1.out_channels, 3, 3, 2, 1)
+        if save is not None:
+            save.x0, save.inv_of, save.layers = x, inv_of, []
+            save.y1 = y
+
+        def norm_act(y, fmt):
+            """lrelu(IN(y)) as a tensor-core operand of `fmt` (+ its fp32 value and IN table when saving)."""
+            if save is None:
+                kw_o, get_o = precision.out_spec(fmt, fmt == ops.BF16)
+                return get_o(ops.instance_norm_act(y, ops.ACT_LRELU, 1e-5, **kw_o)), None, None
+            if fmt == ops.TF32:
+                a32, ss = ops.instance_norm_act_fwd(y, ops.ACT_LRELU, 1e-5, round_out=True)
+                return (ops.TF32, a32, None), a32, ss
+            a32, ss, hi, lo = ops.instance_norm_act_fwd(y, ops.ACT_LRELU, 1e-5, out16=(fmt, True))
+            return (fmt, hi, lo), a32, ss
+
+        for i in range(2, 7):
+            conv = getattr(self, "layer%d" % i)[0]
+            fmt = precision.conv_fmt(y.shape[-1])
+            xo, a32, ss = norm_act(y, fmt)
+            w, isg = weight(conv)
+            wp = precision.pack_conv(w.detach(), isg, fmt)
+            y_next = precision.conv(xo, wp, conv.out_channels, 3, 3, 2, 1)
+            if save is not None:
+                save.layers.append(SimpleNamespace(conv=conv, a=a32, ss=ss, y_in=y))
+            y = y_next
+        # encoder.py:52-57: lrelu(IN(layer6)), flattened; fc_mu | fc_var as one GEMM over the N images
+        K = y[0].numel()
+        fmt = precision.conv_fmt(K)
+        xo, a32, ss = norm_act(y, fmt)
+        xo = (xo[0], xo[1].view(N, 1, 1, K), None if xo[2] is None else xo[2].view(N, 1, 1, K))
+        wf = self.fc_weight()
+        wp = self._cache.get(("fc", fmt), [self.fc_mu.weight, self.fc_var.weight], lambda: precision.pack_conv(wf, None, fmt))
+        bias = self._cache.get("fc_b", [self.fc_mu.bias, self.fc_var.bias],
+                               lambda: torch.cat([self.fc_mu.bias.detach(), self.fc_var.bias.detach()]).contiguous())
+        out = precision.conv(xo, wp, 512, 1, 1, 1, 0, bias=bias).view(N, 512)
+        if save is not None:
+            save.y6, save.ss6, save.a6 = y, ss, a32.view(N, 1, 1, K)
+        return out[:, :256].contiguous(), out[:, 256:].contiguous()

@@ -33,9 +33,9 @@ class SPADEBGenerator(BaseNetwork):
         self.opt = opt
         nf = opt.ngf
         self.sw, self.sh = self.compute_latent_vector_size(opt)
-        if getattr(opt, "use_vae", False) or not opt.use_encoder or opt.Image_encoder_mode != "partialconv":
-            raise NotImplementedError("michigan_b200: spadeb is implemented for --use_encoder with the partialconv "
-                                      "reference encoder (the README configuration)")
+        if not getattr(opt, "use_vae", False) and (not opt.use_encoder or opt.Image_encoder_mode != "partialconv"):
+            raise NotImplementedError("michigan_b200: spadeb is implemented for --use_vae and for --use_encoder with the "
+                                      "partialconv reference encoder (the README configuration)")
         if not opt.noise_background:
             raise NotImplementedError("michigan_b200: spadeb is implemented for --noise_background (BackgroundEncode2)")
         if opt.num_upsampling_layers != "more":
@@ -44,7 +44,13 @@ class SPADEBGenerator(BaseNetwork):
             raise NotImplementedError("michigan_b200: the orientation map is required")
         if getattr(opt, "bf_direct_add", False):
             raise NotImplementedError("michigan_b200: --bf_direct_add is not implemented")
-        self.fc = ImageEncoder3(opt, self.sw, self.sh)
+        if getattr(opt, "use_vae", False):
+            # generator.py:33-35: z -> the 16nf x sh x sw map (run(): one 1x1 GEMM over the N rows of z)
+            if opt.z_dim % 32 != 0:
+                raise NotImplementedError("michigan_b200: z_dim must be a multiple of 32")
+            self.fc = torch.nn.Linear(opt.z_dim, 16 * nf * self.sw * self.sh)
+        else:
+            self.fc = ImageEncoder3(opt, self.sw, self.sh)
         self.head_0 = SPADEResnetBlock(16 * nf, 16 * nf, opt)
         self.G_middle_0 = SPADEResnetBlock(16 * nf, 16 * nf, opt)
         self.G_middle_1 = SPADEResnetBlock(16 * nf, 16 * nf, opt)
@@ -58,6 +64,7 @@ class SPADEBGenerator(BaseNetwork):
         self.backgroud_enc = BackgroundEncode2(opt)  # (sic) the reference's attribute name
         self._blocks = ["head_0", "G_middle_0", "G_middle_1", "up_0", "up_1", "up_2", "up_3"]
         self._snb = None
+        self._cache = PackCache()
         self.last_taps = None
         self.collect_taps = False
 
@@ -104,15 +111,37 @@ class SPADEBGenerator(BaseNetwork):
         opt = self.opt
         if getattr(opt, "orient_random_disturb", False) or getattr(opt, "use_clip", False):
             raise NotImplementedError("michigan_b200: orient_random_disturb / use_clip are debugging paths")
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        grad_z = z is not None and z.requires_grad
+        if torch.is_grad_enabled() and (grad_z or any(p.requires_grad for p in self.parameters())):
             from .autograd import generator_forward_autograd
-            return generator_forward_autograd(self, input, orient_mask, image_ref, input_tag, noise, image_tag)
-        return self.forward_nograd(input, orient_mask, image_ref, input_tag, noise, image_tag)
+            return generator_forward_autograd(self, input, orient_mask, image_ref, input_tag, noise, image_tag, z=z)
+        return self.forward_nograd(input, orient_mask, image_ref, input_tag, noise, image_tag, z=z)
 
-    def forward_nograd(self, input, orient_mask, image_ref, input_tag, noise, image_tag):
-        return self.run(input, orient_mask, image_ref, input_tag, noise, image_tag, None)
+    def forward_nograd(self, input, orient_mask, image_ref, input_tag, noise, image_tag, z=None):
+        return self.run(input, orient_mask, image_ref, input_tag, noise, image_tag, None, z=z)
 
-    def run(self, input, orient_mask, image_ref, input_tag, noise, image_tag, save):
+    def latent_weight(self):
+        """fc.weight [16nf*sh*sw, z_dim] with its rows permuted from the NCHW order (c, h, w) of the reference's view to the
+        NHWC order (h, w, c) of the map head_0 reads, TF32-rounded; and the bias permuted alike (cached until they change)."""
+        def build():
+            hw = self.sh * self.sw
+            w = self.fc.weight.detach().view(-1, hw, self.fc.in_features).transpose(0, 1).reshape(-1, self.fc.in_features, 1, 1)
+            b = self.fc.bias.detach().view(-1, hw).t().contiguous().view(-1)
+            return ops.pack_weight(w.contiguous(), None, True), b
+        return self._cache.get("fc", [self.fc.weight, self.fc.bias], build)
+
+    def latent_head(self, z, N, device, save):
+        """generator.py:110-116: x = view(fc(z)) as [N,sh,sw,16nf] NHWC; z None -> sampled from N(0, I) on the device."""
+        if z is None:
+            z = torch.randn(N, self.opt.z_dim, dtype=torch.float32, device=device)
+        z4 = z.detach().float().contiguous().view(N, 1, 1, -1)
+        wp, b = self.latent_weight()
+        x = ops.conv_igemm(z4, wp, wp.shape[0], 1, 1, 1, 0, bias=b).view(N, self.sh, self.sw, -1)
+        if save is not None:
+            save.z4, save.wp = z4, wp
+        return x
+
+    def run(self, input, orient_mask, image_ref, input_tag, noise, image_tag, save, z=None):
         """The one forward implementation.  save=None: inference / no-grad; save=namespace: the autograd Function's forward,
         which keeps per-block state for the hand-written backward (networks/autograd.py) - identical arithmetic."""
         opt = self.opt
@@ -138,7 +167,10 @@ class SPADEBGenerator(BaseNetwork):
                 bg_done = side.record_event()
         else:
             feats, back = self.backgroud_enc.forward_nhwc(image_tag, input_tag, noise, save=Sbg)  # generator.py:144-147
-        x = self.fc.forward_nhwc(image_ref, ins_ref, ins_tag, save=Sfc)              # generator.py:117-123
+        if getattr(opt, "use_vae", False):
+            x = self.latent_head(z, N, input_tag.device, Sfc)                        # generator.py:110-116
+        else:
+            x = self.fc.forward_nhwc(image_ref, ins_ref, ins_tag, save=Sfc)          # generator.py:117-123
         hair = input_tag[:, 1].contiguous()
         snb = self.spectral_batch()
         inv = snb.run(self.training)

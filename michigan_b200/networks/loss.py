@@ -8,7 +8,7 @@ without --remove_background), evaluated by the fused reduction kernels of csrc/m
 
 The rest of the generator objective follows: the Gabor and DoG orientation losses, VGGLoss / StyleContentLoss (every VGG19 term from one
 pass, _VGGObjectiveFn), LabColorLoss and HairAvgLabLoss (with or without --balance_Lab), RGBBackgroundL1Loss and the rgb L1
-(RGBL1Loss).
+(RGBL1Loss), and the --use_vae KLDLoss.
 """
 import ctypes as C
 import os
@@ -46,6 +46,8 @@ OP_SQ_MASK, OP_MOMENTS = 9, 10
 OP_LAB_BALANCED = 11
 # L1OLoss with the DoG filter: both losses of the batch-normalised confidence and the sums of the gradient through its maximum
 OP_ORIENT_DOG = 12
+# KLDLoss: the logvar half, e^a - a - 1 (the mu half is OP_SQ against zeros)
+OP_KLD_EXP = 13
 MASKED_OPS = (OP_WSUM, OP_HINGE_MASK, OP_L1_MASK, OP_SQ_MASK)      # one scalar term over its own sum(label1) * c + 1e-5
 DEN_EPS = 1e-5          # loss.py:111, 114, 117, 160, 196, 677: sum(label1) * c + 1e-5
 _table_cache = {}
@@ -740,6 +742,20 @@ class StyleContentLoss(nn.Module):
         else:
             _, loss_c, loss_s = vgg_objective(self.vgg, fake_image, content_image, style_image, content=True, style=True)
         return loss_c, loss_s
+
+
+class KLDLoss(nn.Module):
+    """loss.py:211-213: -0.5 sum(1 + logvar - mu^2 - e^logvar), summed over the batch and z, not averaged.  One mg_loss_reduce
+    launch each way with two terms into one slot: 0.5 sum mu^2 (op 3 against zeros) and 0.5 sum (e^logvar - logvar - 1)
+    (op 13), accumulated in fp64.  Under data parallelism each rank sums its own shard, as each DataParallel replica of the
+    reference did before the trainer's mean()."""
+
+    def forward(self, mu, logvar):
+        if mu.shape != logvar.shape:
+            raise ValueError("KLDLoss: mu %s and logvar %s differ in shape" % (tuple(mu.shape), tuple(logvar.shape)))
+        zeros = torch.zeros(mu.shape, device=mu.device, dtype=torch.float32)
+        spec = [_Spec(OP_SQ, 0, zeros, 0.5, 1.0, 0), _Spec(OP_KLD_EXP, 1, None, 0.5, 1.0, 0)]
+        return _LossFn.apply(spec, 1, mu.float(), logvar.float())[0]
 
 
 class _PixelL1Fn(torch.autograd.Function):

@@ -28,7 +28,7 @@ def make_opt(is_train=True, **overrides):
         # loss switches: the stand-alone model implements hinge GAN + GAN_Feat (SURVEY.md §8d flag set)
         no_vgg_loss=True, no_style_loss=True, no_content_loss=True, no_background_loss=True, no_rgb_loss=True, no_lab_loss=True,
         no_orient_loss=True, no_confidence_loss=True, orient_filter="gabor", lambda_orient=10.0, lambda_confidence=100.0,
-        lambda_vgg=1.0, lambda_lab=1.0, balance_Lab=False, lambda_content=1.0, lambda_style=1.0, lambda_background=1.0, lambda_rgb=1.0,
+        lambda_vgg=1.0, lambda_kld=0.05, lambda_lab=1.0, balance_Lab=False, lambda_content=1.0, lambda_style=1.0, lambda_background=1.0, lambda_rgb=1.0,
         isTrain=is_train,
     )
     for k, v in overrides.items():

@@ -13,8 +13,8 @@ import torch
 import torch.nn.functional as F
 
 from . import networks, ops
-from .networks.loss import (GANFeatLoss, GANLoss, LabColorLoss, RGBBackgroundL1Loss, RGBL1Loss, StyleContentLoss, VGGLoss,
-                            vgg_objective)
+from .networks.loss import (GANFeatLoss, GANLoss, KLDLoss, LabColorLoss, RGBBackgroundL1Loss, RGBL1Loss, StyleContentLoss,
+                            VGGLoss, vgg_objective)
 
 
 class Pix2PixModel(torch.nn.Module):
@@ -28,7 +28,7 @@ class Pix2PixModel(torch.nn.Module):
         self.opt = opt
         if len(opt.gpu_ids) == 0:
             raise RuntimeError("michigan_b200 has no CPU path: gpu_ids must name a CUDA device")
-        for flag in ("use_vae", "use_blender", "use_instance_feat", "unpairTrain"):
+        for flag in ("use_blender", "use_instance_feat", "unpairTrain"):
             if getattr(opt, flag, False):
                 raise NotImplementedError("michigan_b200: --%s is outside the hot path (SURVEY.md §8)" % flag)
         # Every term of the reference's generator objective for curr_step 1 (pix2pix_model.py:296-345) is computed here: GAN
@@ -42,7 +42,12 @@ class Pix2PixModel(torch.nn.Module):
             self._load_inpainting_network(opt)
         self.netG = networks.define_G(opt)
         self.netD = networks.define_D(opt) if opt.isTrain else None
+        # --use_vae (pix2pix_model.py:42-43, 172): netE encodes image_ref to (mu, logvar), z = mu + eps exp(logvar / 2) drives
+        # the generator's latent head, and the G step adds KLD first in G_losses
+        self.netE = networks.define_E(opt) if getattr(opt, "use_vae", False) else None
         if opt.isTrain:
+            if self.netE is not None:
+                self.KLDLoss = KLDLoss()
             self.criterionGAN = GANLoss(opt.gan_mode, opt=opt)
             self.criterionGANFeat = GANFeatLoss(opt)
             if not getattr(opt, "no_vgg_loss", False):
@@ -76,14 +81,19 @@ class Pix2PixModel(torch.nn.Module):
             load_weights(self.netG, torch.load(path, map_location="cpu"))
             if opt.isTrain and os.path.exists(self._ckpt_path("D", epoch)):
                 load_weights(self.netD, torch.load(self._ckpt_path("D", epoch), map_location="cpu"))
+            if self.netE is not None:
+                load_weights(self.netE, torch.load(self._ckpt_path("E", epoch), map_location="cpu"))
 
     def save(self, epoch):
-        """<checkpoints_dir>/<name>/<epoch>_net_{G,D}.pth, CPU state dicts with the reference's keys (util.py:195-200):
+        """<checkpoints_dir>/<name>/<epoch>_net_{G,D,E}.pth (E with --use_vae, pix2pix_model.py:157-158), CPU state dicts with
+        the reference's keys (util.py:195-200):
         rank 0 writes (snapshot copied on a side stream, serialised by a background thread), all ranks meet at a barrier."""
         from . import checkpoint
         checkpoint.save_state_dict(self.netG, self._ckpt_path("G", epoch))
         if self.netD is not None:
             checkpoint.save_state_dict(self.netD, self._ckpt_path("D", epoch))
+        if self.netE is not None:
+            checkpoint.save_state_dict(self.netE, self._ckpt_path("E", epoch))
 
     def _load_inpainting_network(self, opt):
         """util.load_inpainting_network (util.py:245-257): <checkpoints_dir>/<name>/<ig_model_name> = {'generator': state_dict}."""
@@ -125,6 +135,9 @@ class Pix2PixModel(torch.nn.Module):
             return self.compute_generator_loss(input_ref, input_tag, image_ref, image_tag, orient_mask, noise)
         if mode == "discriminator":
             return self.compute_discriminator_loss(input_ref, input_tag, image_ref, image_tag, orient_mask, noise)
+        if mode == "encode_only":
+            _, mu, logvar = self.encode_z(image_ref)
+            return mu, logvar
         if mode == "inference":
             with torch.no_grad():
                 return self.generate_fake(input_ref, image_ref, orient_mask, input_tag, image_tag, noise)
@@ -132,6 +145,8 @@ class Pix2PixModel(torch.nn.Module):
 
     def create_optimizers(self, opt):
         G_params = list(self.netG.parameters())
+        if self.netE is not None:
+            G_params += list(self.netE.parameters())
         D_params = list(self.netD.parameters()) if opt.isTrain else []
         if opt.no_TTUR:
             beta1, beta2 = opt.beta1, opt.beta2
@@ -168,11 +183,22 @@ class Pix2PixModel(torch.nn.Module):
         out[:, :, o:o + H, o:o + W] = t
         return out
 
-    def generate_fake(self, input_ref, image_ref, orient_mask, input_tag, image_tag, noise):
+    def encode_z(self, real_image):
+        """pix2pix_model.py:400-403, 604-607: (z, mu, logvar).  The reparameterisation acts on N x 256 elements and stays torch
+        arithmetic, as the reference's own Pix2PixModel.reparameterize does when install() drives it."""
+        mu, logvar = self.netE(real_image)
+        std = torch.exp(0.5 * logvar)
+        eps = torch.randn_like(std)
+        return eps.mul(std) + mu, mu, logvar
+
+    def generate_fake(self, input_ref, image_ref, orient_mask, input_tag, image_tag, noise, z=None):
+        """pix2pix_model.py:505-541; with --use_vae and no z given, z is encoded from image_ref (every mode, as the reference)."""
+        if self.netE is not None and z is None:
+            z, _, _ = self.encode_z(image_ref.clone())
         if self.opt.add_feat_zeros:
             input_ref, image_ref, orient_mask, input_tag, image_tag, noise = [
                 self.zeros_padding(t) for t in (input_ref, image_ref, orient_mask, input_tag, image_tag, noise)]
-        return self.netG(input_ref, z=None, orient_mask=orient_mask, image_ref=image_ref, input_tag=input_tag, noise=noise,
+        return self.netG(input_ref, z=z, orient_mask=orient_mask, image_ref=image_ref, input_tag=input_tag, noise=noise,
                          image_tag=image_tag)
 
     def discriminate(self, input_tag, fake_image, real_image, orient_mask):
@@ -188,7 +214,12 @@ class Pix2PixModel(torch.nn.Module):
 
     def compute_generator_loss(self, input_ref, input_tag, image_ref, image_tag, orient_mask, noise):
         G_losses = {}
-        fake_image = self.generate_fake(input_ref, image_ref, orient_mask, input_tag, image_tag, noise)
+        z = None
+        if self.netE is not None:
+            # pix2pix_model.py:266-271, 505-511: KLD is the first key
+            z, mu, logvar = self.encode_z(image_ref.clone())
+            G_losses["KLD"] = self.KLDLoss(mu, logvar) * self.opt.lambda_kld
+        fake_image = self.generate_fake(input_ref, image_ref, orient_mask, input_tag, image_tag, noise, z=z)
         # The discriminator's parameters are constants of the generator's objective: the reference back-propagates into
         # them anyway and discards the result (optimizer_D.zero_grad() precedes their only use, pix2pix_trainer.py:62-69).
         with _frozen(self.netD):
