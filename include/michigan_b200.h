@@ -218,7 +218,9 @@ int mg_avgpool3s2(const float* in, float* out, int N, int H, int W, int C, int O
 /* PartialConv2d mask update (partialconv2d.py:57-66): mask [N,H,W] -> ratio, update [N,OH,OW]. */
 int mg_partial_mask(const float* mask, float* ratio, float* update, int N, int H, int W, int k, int stride, int pad,
                     void* stream);
-/* ImageEncoder3 instance-wise average pooling (encoder.py:207-220); masks are [N,MH,MW] full-res. */
+/* ImageEncoder3 / ImageEncoder2 instance-wise average pooling (encoder.py:142-151, 207-220); masks are [N,MH,MW] full-res,
+   MH, MW multiples of h, w.  mref == NULL: the plain spatial mean (denominator h*w: --ref_global_pool, AdaptiveAvgPool2d(1));
+   mtag == NULL: broadcast with weight 1.  MH, MW are read only when a mask is given.  The backward takes the same modes. */
 int mg_masked_mean_bcast(const float* x, const float* mref, const float* mtag, float* out, int N, int h, int w, int C,
                          int MH, int MW, void* stream);
 /* F.interpolate(bilinear, align_corners=False) on NHWC (encoder.py:222-223). */

@@ -761,9 +761,11 @@ __global__ void partial_mask_kernel(const float* __restrict__ mask, float* __res
     }
 }
 
-// ImageEncoder3 tail (encoder.py:207-220): per sample, mean of x over the reference-hair pixels
+// ImageEncoder3 / ImageEncoder2 tail (encoder.py:142-151, 207-220): per sample, mean of x over the reference-hair pixels
 // (sum / max(count,1)), broadcast onto the target-hair pixels.  Masks are full-resolution [N,MH,MW]
-// read through the legacy nearest resize (index * MH/h).  One block per (n, 32-channel group).
+// read through the legacy nearest resize (index * MH/h).  mref == NULL: every pixel weighs 1, so the mean is the plain
+// spatial mean (denominator h*w; --ref_global_pool, AdaptiveAvgPool2d(1)); mtag == NULL: broadcast with weight 1.
+// One block per (n, 32-channel group).
 __global__ void masked_mean_bcast_kernel(const float* __restrict__ x, const float* __restrict__ mref,
                                          const float* __restrict__ mtag, float* __restrict__ out, int N, int h, int w,
                                          int C, int MH, int MW) {
@@ -776,7 +778,7 @@ __global__ void masked_mean_bcast_kernel(const float* __restrict__ x, const floa
     float acc = 0.f, cnt = 0.f;
     for (int pidx = row; pidx < h * w; pidx += 8) {
         const int ph = pidx / w, pw = pidx - ph * w;
-        const float m = mref[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw];
+        const float m = mref ? mref[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw] : 1.f;
         cnt += m;
         if (c < C) acc += x[(((size_t)n * h + ph) * w + pw) * C + c] * m;
     }
@@ -788,7 +790,7 @@ __global__ void masked_mean_bcast_kernel(const float* __restrict__ x, const floa
     const float mean = tot / fmaxf(ctot, 1.f);
     for (int pidx = row; pidx < h * w; pidx += 8) {
         const int ph = pidx / w, pw = pidx - ph * w;
-        const float m = mtag[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw];
+        const float m = mtag ? mtag[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw] : 1.f;
         if (c < C) out[(((size_t)n * h + ph) * w + pw) * C + c] = mean * m;
     }
 }
@@ -1127,8 +1129,9 @@ extern "C" int mg_partial_mask(const float* mask, float* ratio, float* update, i
 }
 extern "C" int mg_masked_mean_bcast(const float* x, const float* mref, const float* mtag, float* out, int N, int h, int w,
                                     int C, int MH, int MW, void* stream) {
-    if (!x || !mref || !mtag || !out) return set_error(-1, "mg_masked_mean_bcast: null pointer");
-    if (MH % h != 0 || MW % w != 0) return set_error(-2, "mg_masked_mean_bcast: mask size must be a multiple of the map size");
+    if (!x || !out) return set_error(-1, "mg_masked_mean_bcast: null pointer");
+    if ((mref || mtag) && (h <= 0 || w <= 0 || MH % h != 0 || MW % w != 0))
+        return set_error(-2, "mg_masked_mean_bcast: mask size must be a multiple of the map size");
     dim3 grid(cdiv(C, 32), N);
     masked_mean_bcast_kernel<<<grid, 256, 0, ST(stream)>>>(x, mref, mtag, out, N, h, w, C, MH, MW);
     return check_launch("mg_masked_mean_bcast");

@@ -807,7 +807,7 @@ __global__ void resize_bilinear_bwd_kernel(const float* __restrict__ dout, doubl
     }
 }
 // masked mean broadcast backward: out[p,c] = mean_c * mtag[p], mean_c = sum_q x[q,c]*mref[q] / max(cnt,1)
-//  => dx[q,c] = mref[q]/max(cnt,1) * sum_p dout[p,c]*mtag[p]
+//  => dx[q,c] = mref[q]/max(cnt,1) * sum_p dout[p,c]*mtag[p].  A NULL mask weighs every pixel 1, as in the forward.
 __global__ void masked_mean_bcast_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ mref,
                                              const float* __restrict__ mtag, float* __restrict__ dx, int N, int h, int w, int C,
                                              int MH, int MW) {
@@ -820,8 +820,8 @@ __global__ void masked_mean_bcast_bwd_kernel(const float* __restrict__ dout, con
     float acc = 0.f, cnt = 0.f;
     for (int pidx = row; pidx < h * w; pidx += 8) {
         const int ph = pidx / w, pw = pidx - ph * w;
-        cnt += mref[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw];
-        const float mt = mtag[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw];
+        cnt += mref ? mref[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw] : 1.f;
+        const float mt = mtag ? mtag[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw] : 1.f;
         if (c < C) acc += dout[(((size_t)n * h + ph) * w + pw) * C + c] * mt;
     }
     red[row][threadIdx.x & 31] = acc;
@@ -832,7 +832,7 @@ __global__ void masked_mean_bcast_bwd_kernel(const float* __restrict__ dout, con
     const float gmean = tot / fmaxf(ctot, 1.f);
     for (int pidx = row; pidx < h * w; pidx += 8) {
         const int ph = pidx / w, pw = pidx - ph * w;
-        const float m = mref[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw];
+        const float m = mref ? mref[((size_t)n * MH + (size_t)ph * sh) * MW + (size_t)pw * sw] : 1.f;
         if (c < C) dx[(((size_t)n * h + ph) * w + pw) * C + c] = gmean * m;
     }
 }
@@ -1134,7 +1134,9 @@ extern "C" int mg_resize_bilinear_bwd(const float* dout, float* din_zeroed, int 
 }
 extern "C" int mg_masked_mean_bcast_bwd(const float* dout, const float* mref, const float* mtag, float* dx, int N, int h, int w, int C,
                                         int MH, int MW, void* stream) {
-    if (!dout || !mref || !mtag || !dx) return set_error(-1, "mg_masked_mean_bcast_bwd: null pointer");
+    if (!dout || !dx) return set_error(-1, "mg_masked_mean_bcast_bwd: null pointer");
+    if ((mref || mtag) && (h <= 0 || w <= 0 || MH % h != 0 || MW % w != 0))
+        return set_error(-2, "mg_masked_mean_bcast_bwd: mask size must be a multiple of the map size");
     dim3 grid(cdivb(C, 32), N);
     masked_mean_bcast_bwd_kernel<<<grid, 256, 0, ST(stream)>>>(dout, mref, mtag, dx, N, h, w, C, MH, MW);
     return check_launch("mg_masked_mean_bcast_bwd");

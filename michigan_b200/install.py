@@ -46,6 +46,8 @@ def install(reference_root=None, compat=True):
     gen.SPADEBGenerator = G
     gen.SPADEResnetBlock = mine.SPADEResnetBlock
     gen.ImageEncoder3 = mine.ImageEncoder3
+    gen.ImageEncoder = mine.ImageEncoder
+    gen.ImageEncoder2 = mine.ImageEncoder2
     gen.BackgroundEncode2 = mine.BackgroundEncode2
     dis.MultiscaleDiscriminator = MSD
     dis.NLayerDiscriminator = NLD
@@ -54,6 +56,8 @@ def install(reference_root=None, compat=True):
     arc.SPADEResnetBlock = mine.SPADEResnetBlock
     arc.SPADE = mine.SPADE
     enc.ImageEncoder3 = mine.ImageEncoder3
+    enc.ImageEncoder = mine.ImageEncoder
+    enc.ImageEncoder2 = mine.ImageEncoder2
     enc.BackgroundEncode2 = mine.BackgroundEncode2
     # --use_vae: define_E finds 'convencoder' in models.networks.encoder (networks/__init__.py:65-68)
     enc.ConvEncoder = both(mine.ConvEncoder)

@@ -8,7 +8,7 @@ from .normalization import SPADE, get_nonspade_norm_layer
 from .architecture import SPADEResnetBlock, VGG19
 from . import loss
 from .loss import GANLoss, GANFeatLoss, VGGLoss, LabColorLoss, StyleContentLoss, RGBBackgroundL1Loss, HairAvgLabLoss, KLDLoss
-from .encoder import ImageEncoder3, BackgroundEncode2, PartialConv2d, ConvBlock, ConvEncoder
+from .encoder import ImageEncoder, ImageEncoder2, ImageEncoder3, BackgroundEncode2, PartialConv2d, ConvBlock, ConvEncoder
 from .generator import SPADEBGenerator
 from .discriminator import MultiscaleDiscriminator, NLayerDiscriminator
 from .inpaint import InpaintGenerator

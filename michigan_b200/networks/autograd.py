@@ -1,5 +1,6 @@
 """Training path: hand-written backward passes wired into torch.autograd as three Functions
-(generator, multiscale discriminator, the --use_vae ConvEncoder).  Forward = the networks' ONE forward implementation (`SPADEBGenerator.run`,
+(generator, multiscale discriminator, the --use_vae ConvEncoder); the generator's reference-image encoder is reached through
+its backward_nhwc method.  Forward = the networks' ONE forward implementation (`SPADEBGenerator.run`,
 `MultiscaleDiscriminator.run`) in "save" mode: the same kernels and operand formats as inference (precision.py), which
 additionally keep the fp32 value of every tensor the gradient GEMMs need (read as TF32 by the wgrad / dgrad kernels);
 backward = explicit reverse pass over the saved per-block state:
@@ -182,12 +183,12 @@ def bg_bwd(G, bg, S, dfeats):
 
 
 def latent_bwd(G, fc, S, dx):
-    """Backward of the --use_vae latent head x = view(z W^T + b) (generator.py:110-116) given dx [N,sh,sw,16nf] NHWC;
-    returns dz [N, z_dim].  The weight and bias gradients read dx in the reference's NCHW row order (one transpose of the
-    N x 16nf*sh*sw gradient), so they come out in fc.weight's own layout.  They are one weight-gradient GEMM over the N rows:
-    z is extended by a column of ones (the bias) and 31 zeros (the GEMM's 32-column granule), so dW | db = dY^T [z | 1 | 0]
-    (the per-channel sum kernels take at most 4096 channels; the head has 16nf*sh*sw).  dz is the 1x1 data-gradient GEMM on
-    the permuted weight the forward packed (S.wp)."""
+    """Backward of encoder.latent_head, x = view(z W^T + b): the --use_vae head (generator.py:110-116) and ImageEncoder's fc
+    (encoder.py:99-101), given dx [N,sh,sw,C] NHWC; returns dz [N, K].  The weight and bias gradients read dx in the
+    reference's NCHW row order (one transpose of the N x C*sh*sw gradient), so they come out in fc.weight's own layout.  They
+    are one weight-gradient GEMM over the N rows: z is extended by a column of ones (the bias) and 31 zeros (the GEMM's
+    32-column granule), so dW | db = dY^T [z | 1 | 0] (the per-channel sum kernels take at most 4096 channels; the head has
+    C*sh*sw).  dz is the 1x1 data-gradient GEMM on the permuted weight the forward packed (S.wp)."""
     N = dx.shape[0]
     K = dx[0].numel()
     dy_ref = ops.nhwc_to_nchw(dx).view(N, 1, 1, K)
@@ -237,7 +238,7 @@ class _GeneratorFn(torch.autograd.Function):
             if not ctx.needs_input_grad[1]:
                 dz = None
         else:
-            fc_bwd(G, netG.fc, ctx.Sfc, dx)
+            netG.fc.backward_nhwc(G, ctx.Sfc, dx)
         bg_bwd(G, netG.backgroud_enc, ctx.Sbg, dfeats)
         ctx.saved = ctx.Sfc = ctx.Sbg = None
         if red is not None:
@@ -252,9 +253,24 @@ def generator_forward_autograd(netG, input_ref, orient_mask, image_ref, input_ta
 
 
 # =============================================================================================== ConvEncoder Function
+def sn_conv_stack_bwd(G, convs, S, dy):
+    """Parameter gradients of encoder.SNConvStack.run_stack given dy, the TF32-rounded gradient of its output: its SN conv +
+    InstanceNorm + LeakyReLU layers in reverse, as _d_scale_bwd does for the discriminator's convs.  convs: the stack's
+    convs(); S: the namespace run_stack filled."""
+    for L in reversed(S.layers):
+        _conv_param_grads(G, L.conv, S.inv_of, dy, L.a, 3, 3, 2, 1, with_bias=False)
+        w, isg, _ = _conv_weight(L.conv, S.inv_of)
+        da = ops.conv_dgrad(dy, w.detach(), (L.a.shape[1], L.a.shape[2]), 2, 1, inv_sigma=isg)
+        dy = ops.in_bwd(da, L.y_in, L.ss, _LRELU, round_tf32=L is not S.layers[0])
+    conv1 = convs[0]
+    w1, isg1, is_sn = _conv_weight(conv1, S.inv_of)
+    dwt = _thin_wt_to_oihw(ops.thin_wgrad(S.x0, dy, 3, 3, 2, 1), 3, 3, 3)
+    G.add(w1, ops.spectral_norm_bwd(dwt, w1.detach(), conv1.weight_u, conv1.weight_v, isg1) if is_sn else dwt)
+
+
 def conv_encoder_bwd(G, E, S, dout):
     """Parameter gradients of ConvEncoder.run given dout = d(mu | logvar) [N,1,1,512]: fc_mu | fc_var weight and bias, then the
-    six SN conv + InstanceNorm + LeakyReLU layers in reverse, as _d_scale_bwd does for the discriminator's convs."""
+    six layers of the stack (sn_conv_stack_bwd)."""
     N = dout.shape[0]
     dwf = ops.conv_wgrad(dout, S.a6, 1, 1, 1, 0)                  # [512, 16C], columns in the map's NHWC order
     c = S.y6.shape[-1]
@@ -265,16 +281,7 @@ def conv_encoder_bwd(G, E, S, dout):
     G.add(E.fc_mu.bias, db[:256])
     G.add(E.fc_var.bias, db[256:])
     da = ops.conv_dgrad(dout, E.fc_weight(), (1, 1), 1, 0).view(S.y6.shape)
-    dy = ops.in_bwd(da, S.y6, S.ss6, _LRELU, round_tf32=True)
-    for L in reversed(S.layers):
-        _conv_param_grads(G, L.conv, S.inv_of, dy, L.a, 3, 3, 2, 1, with_bias=False)
-        w, isg, _ = _conv_weight(L.conv, S.inv_of)
-        da = ops.conv_dgrad(dy, w.detach(), (L.a.shape[1], L.a.shape[2]), 2, 1, inv_sigma=isg)
-        dy = ops.in_bwd(da, L.y_in, L.ss, _LRELU, round_tf32=L is not S.layers[0])
-    conv1 = E.layer1[0]
-    w1, isg1, is_sn = _conv_weight(conv1, S.inv_of)
-    dwt = _thin_wt_to_oihw(ops.thin_wgrad(S.x0, dy, 3, 3, 2, 1), 3, 3, 3)
-    G.add(w1, ops.spectral_norm_bwd(dwt, w1.detach(), conv1.weight_u, conv1.weight_v, isg1) if is_sn else dwt)
+    sn_conv_stack_bwd(G, E.convs(), S, ops.in_bwd(da, S.y6, S.ss6, _LRELU, round_tf32=True))
 
 
 class _ConvEncoderFn(torch.autograd.Function):

@@ -14,12 +14,16 @@ import torch
 from .. import ops
 from .architecture import SPADEResnetBlock
 from .base_network import BaseNetwork
-from .encoder import BackgroundEncode2, ImageEncoder3
+from .encoder import BackgroundEncode2, ImageEncoder, ImageEncoder2, ImageEncoder3, latent_head
 from .prep import PackCache, SpectralNormBatch
 
 # MICHIGAN_B200_OVERLAP=1: background encoder on a second stream (off by default: the low-resolution blocks are short and the
 # encoder's one-CTA-per-SM kernels cannot share an SM with a large-smem GEMM CTA anyway).
 _OVERLAP = os.environ.get("MICHIGAN_B200_OVERLAP", "0") == "1"
+
+
+# --Image_encoder_mode -> the reference-image encoder of --use_encoder (generator.py:38-44)
+IMAGE_ENCODERS = {"partialconv": ImageEncoder3, "instance": ImageEncoder2, "norm": ImageEncoder}
 
 
 class SPADEBGenerator(BaseNetwork):
@@ -33,9 +37,13 @@ class SPADEBGenerator(BaseNetwork):
         self.opt = opt
         nf = opt.ngf
         self.sw, self.sh = self.compute_latent_vector_size(opt)
-        if not getattr(opt, "use_vae", False) and (not opt.use_encoder or opt.Image_encoder_mode != "partialconv"):
-            raise NotImplementedError("michigan_b200: spadeb is implemented for --use_vae and for --use_encoder with the "
-                                      "partialconv reference encoder (the README configuration)")
+        if not getattr(opt, "use_vae", False):
+            if not opt.use_encoder:
+                raise NotImplementedError("michigan_b200: spadeb is implemented for --use_vae and for --use_encoder (the "
+                                          "deterministic head has no kernels)")
+            if opt.Image_encoder_mode not in IMAGE_ENCODERS:
+                raise NotImplementedError("michigan_b200: --Image_encoder_mode '%s' is not one of %s"
+                                          % (opt.Image_encoder_mode, ", ".join(IMAGE_ENCODERS)))
         if not opt.noise_background:
             raise NotImplementedError("michigan_b200: spadeb is implemented for --noise_background (BackgroundEncode2)")
         if opt.num_upsampling_layers != "more":
@@ -50,7 +58,7 @@ class SPADEBGenerator(BaseNetwork):
                 raise NotImplementedError("michigan_b200: z_dim must be a multiple of 32")
             self.fc = torch.nn.Linear(opt.z_dim, 16 * nf * self.sw * self.sh)
         else:
-            self.fc = ImageEncoder3(opt, self.sw, self.sh)
+            self.fc = IMAGE_ENCODERS[opt.Image_encoder_mode](opt, self.sw, self.sh)
         self.head_0 = SPADEResnetBlock(16 * nf, 16 * nf, opt)
         self.G_middle_0 = SPADEResnetBlock(16 * nf, 16 * nf, opt)
         self.G_middle_1 = SPADEResnetBlock(16 * nf, 16 * nf, opt)
@@ -120,26 +128,12 @@ class SPADEBGenerator(BaseNetwork):
     def forward_nograd(self, input, orient_mask, image_ref, input_tag, noise, image_tag, z=None):
         return self.run(input, orient_mask, image_ref, input_tag, noise, image_tag, None, z=z)
 
-    def latent_weight(self):
-        """fc.weight [16nf*sh*sw, z_dim] with its rows permuted from the NCHW order (c, h, w) of the reference's view to the
-        NHWC order (h, w, c) of the map head_0 reads, TF32-rounded; and the bias permuted alike (cached until they change)."""
-        def build():
-            hw = self.sh * self.sw
-            w = self.fc.weight.detach().view(-1, hw, self.fc.in_features).transpose(0, 1).reshape(-1, self.fc.in_features, 1, 1)
-            b = self.fc.bias.detach().view(-1, hw).t().contiguous().view(-1)
-            return ops.pack_weight(w.contiguous(), None, True), b
-        return self._cache.get("fc", [self.fc.weight, self.fc.bias], build)
-
     def latent_head(self, z, N, device, save):
-        """generator.py:110-116: x = view(fc(z)) as [N,sh,sw,16nf] NHWC; z None -> sampled from N(0, I) on the device."""
+        """generator.py:110-116: x = view(fc(z)) as [N,sh,sw,16nf] NHWC (encoder.latent_head); z None -> sampled from
+        N(0, I) on the device."""
         if z is None:
             z = torch.randn(N, self.opt.z_dim, dtype=torch.float32, device=device)
-        z4 = z.detach().float().contiguous().view(N, 1, 1, -1)
-        wp, b = self.latent_weight()
-        x = ops.conv_igemm(z4, wp, wp.shape[0], 1, 1, 1, 0, bias=b).view(N, self.sh, self.sw, -1)
-        if save is not None:
-            save.z4, save.wp = z4, wp
-        return x
+        return latent_head(self._cache, self.fc, z, self.sh, self.sw, save)
 
     def run(self, input, orient_mask, image_ref, input_tag, noise, image_tag, save, z=None):
         """The one forward implementation.  save=None: inference / no-grad; save=namespace: the autograd Function's forward,

@@ -420,12 +420,23 @@ def partial_mask(mask, k, stride, pad):
     return ratio, upd
 
 
+def _mask_hw(mref, mtag, h, w):
+    """(MH, MW) of the full-resolution masks of masked_mean_bcast[_bwd]; both must match.  No mask: the map's own size."""
+    hw = [tuple(m.shape[-2:]) for m in (mref, mtag) if m is not None]
+    if len(set(hw)) > 1:
+        raise ValueError("masked_mean_bcast: mref and mtag differ in size: %s" % (hw,))
+    return hw[0] if hw else (h, w)
+
+
 def masked_mean_bcast(x, mref, mtag):
+    """out[n,p,c] = mtag[n,p] * sum_q x[n,q,c] mref[n,q] / max(sum_q mref[n,q], 1) on NHWC x, masks [N,MH,MW] read at stride
+    MH/h.  mref None: the plain spatial mean; mtag None: broadcast with weight 1."""
     _chk(x, "x"); _chk(mref, "mref"); _chk(mtag, "mtag")
     N, h, w, Cc = x.shape
+    MH, MW = _mask_hw(mref, mtag, h, w)
     out = torch.empty_like(x)
-    check(_lib.load().mg_masked_mean_bcast(_p(x), _p(mref), _p(mtag), _p(out), N, h, w, Cc, mref.shape[-2],
-                                           mref.shape[-1], _stream()), "mg_masked_mean_bcast")
+    check(_lib.load().mg_masked_mean_bcast(_p(x), _p(mref), _p(mtag), _p(out), N, h, w, Cc, MH, MW, _stream()),
+          "mg_masked_mean_bcast")
     return out
 
 
@@ -912,11 +923,13 @@ def resize_bilinear_bwd(dout, in_hw):
 
 
 def masked_mean_bcast_bwd(dout, mref, mtag):
+    """Gradient of masked_mean_bcast w.r.t. x, with the same None modes."""
     _chk(dout, "dout"); _chk(mref, "mref"); _chk(mtag, "mtag")
     N, h, w, Cc = dout.shape
+    MH, MW = _mask_hw(mref, mtag, h, w)
     dx = torch.empty_like(dout)
-    check(_lib.load().mg_masked_mean_bcast_bwd(_p(dout), _p(mref), _p(mtag), _p(dx), N, h, w, Cc, mref.shape[-2], mref.shape[-1],
-                                               _stream()), "mg_masked_mean_bcast_bwd")
+    check(_lib.load().mg_masked_mean_bcast_bwd(_p(dout), _p(mref), _p(mtag), _p(dx), N, h, w, Cc, MH, MW, _stream()),
+          "mg_masked_mean_bcast_bwd")
     return dx
 
 

@@ -14,7 +14,7 @@ def make_opt(is_train=True, **overrides):
         aspect_ratio=1.0, label_nc=2, contain_dontcare_label=False, output_nc=3, orient_nc=2, netG="spadeb", ngf=64,
         init_type="xavier", init_variance=0.02, z_dim=256, use_ig=False, num_upsampling_layers="more",
         use_instance_feat=False, feat_num=3, use_encoder=True, Image_encoder_mode="partialconv",
-        norm_ref_encode="instance", use_blender=False, no_instance=True, use_vae=False, noise_background=True,
+        ref_global_pool=False, norm_ref_encode="instance", use_blender=False, no_instance=True, use_vae=False, noise_background=True,
         random_expand_mask=True, random_expand_th=0.05, bf_direct_add=False, random_noise_background=False,
         no_orientation=False, add_feat_zeros=False, add_th=64, clip_th=300, use_clip=False, orient_random_disturb=False,
         expand_mask_be=True, expand_th=5, semantic_nc=2, inpaint_mode="ref", only_blend=False, unpairTrain=False,
