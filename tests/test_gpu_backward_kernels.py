@@ -23,11 +23,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64ref import TINY, U, check_close, d64, nchw, nhwc, rna_tf32, vjp64
+
 pytestmark = pytest.mark.gpu
 dev = "cuda"
-
-U = 2.0 ** -24        # fp32 unit roundoff
-TINY = 1e-30
 
 
 @pytest.fixture(autouse=True)
@@ -53,52 +52,6 @@ def _ops():
 def _lib():
     from michigan_b200 import _lib
     return _lib
-
-
-def tf32_trunc(t):
-    return (t.view(torch.int32) & ~0x1FFF).view(torch.float32)
-
-
-def rna_tf32(t):
-    """cvt.rna.tf32.f32 on finite fp32 values: round the magnitude to 10 stored mantissa bits, ties away from zero."""
-    return ((t.view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
-
-
-def nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
-
-
-def d64(t):
-    return t.detach().cpu().double()
-
-
-def vjp64(fn, inputs, dout):
-    """fp64 CPU autograd: -> (fn(*inputs), d inputs) for the output gradient dout."""
-    xs = [d64(t).requires_grad_(True) for t in inputs]
-    out = fn(*xs)
-    gs = torch.autograd.grad(out, xs, d64(dout), allow_unused=True)
-    return out.detach(), gs
-
-
-def check_close(name, got, ref, rabs, k, u=U, skip=None):
-    """|got - ref| <= k * u * rabs + TINY for every element (skip: boolean mask of elements left out)."""
-    got, ref, rabs = d64(got), d64(ref), d64(rabs)
-    assert got.shape == ref.shape == rabs.shape, (name, got.shape, ref.shape, rabs.shape)
-    assert bool(torch.isfinite(got).all()), name
-    err = (got - ref).abs()
-    if skip is not None:
-        err = torch.where(skip, torch.zeros_like(err), err)
-    ratio = float((err / (u * rabs + TINY)).max())
-    print("%s: max |got - ref| / (u R_abs) = %.3g (k = %g)" % (name, ratio, k))
-    bad = err > k * u * rabs + TINY
-    if bool(bad.any()):
-        i = tuple(bad.nonzero()[0].tolist())
-        raise AssertionError("%s: %d of %d elements out of bound; max ratio %.3g > k = %g; first at %s: got %r ref %r R_abs %r"
-                             % (name, int(bad.sum()), bad.numel(), ratio, k, i, float(got[i]), float(ref[i]), float(rabs[i])))
 
 
 def check_rounded(name, got, ref, rabs, bits, k):

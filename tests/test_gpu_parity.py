@@ -281,8 +281,9 @@ def test_backward_chain_smooth_loss_vs_oracle():
     D is compared in relative L2.  Bound: 0.1 (measured <= 4e-2; round 1: 0.2).  The forward runs with TF32 operands (features accurate to
     ~5e-4), and LeakyReLU / ReLU derivatives jump at 0, so ~0.05 % of the activation-derivative masks differ
     from the fp32 oracle per layer: measured ~2e-2 per discriminator layer, ~1e-2 per SPADE block, compounding
-    to ~0.12 at the reference encoder (7 blocks upstream); single-block and single-kernel gradients are checked
-    to 1e-2 / 5e-5 by tools/debug_bwd.py and tools/probe_kernels.py bwd2.  Tensors whose reference
+    to ~0.12 at the reference encoder (7 blocks upstream).  Each backward stage on its own (every SPADE block, the
+    encoders, the discriminator scales) is held to float64 autograd element by element, at the forward's own activation
+    masks, by tests/test_gpu_backward_stages_fp64.py.  Tensors whose reference
     norm is below 1e-4 (1e-2 for 1-D sums) of the largest are measured against that floor."""
     from michigan_b200 import networks
     from michigan_b200.options import make_opt

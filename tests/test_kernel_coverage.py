@@ -5,6 +5,9 @@ exercises one when its code (not its comments or docstrings) names the entry poi
 (directly or through other ops.* functions), or a top-level class / function of the package that reaches it (e.g.
 SpectralNormBatch, LabColorLoss; not a whole network, see END_TO_END).  Package names count only as the module's imports
 bind them.  Entry points no such module reaches are listed in NOT_IN_GPU_TESTS with the reason.
+
+Every hand-written backward function of the training path is reached by tests/test_gpu_backward_stages_fp64.py, which holds
+each stage to float64 autograd element by element; functions deliberately left out are listed in NOT_IN_BACKWARD_STAGES.
 """
 import ast
 import os
@@ -48,9 +51,21 @@ ELEMENTWISE_TESTS = {
 NOT_ELEMENTWISE = {}
 
 
+# The module that holds every hand-written backward stage to float64 autograd, and the backward functions it leaves out.
+BACKWARD_STAGES_MODULE = "test_gpu_backward_stages_fp64.py"
+NOT_IN_BACKWARD_STAGES = {
+    "_GeneratorFn.backward": "chains conv_img_bwd (test_gpu_backward_kernels.py) and the stages block_bwd, latent_bwd, "
+                             "backward_nhwc and bg_bwd, each tested on its own; end to end in test_gpu_parity.py",
+    "_ConvEncoderFn.backward": "concatenates d mu | d logvar and calls conv_encoder_bwd, which is tested; end to end in "
+                               "test_gpu_vae.py",
+}
+
+
 # Whole networks and the training model run dozens of kernels end to end, under bounds loose enough to pass a kernel that is
 # wrong on one border or channel range: reaching an entry point only through one of them does not count.
 END_TO_END = {"BaseNetwork", "Pix2PixModel"}
+# Code that runs only across two or more ranks (single-process callers return before reaching it): reaching it credits nothing.
+MULTI_RANK = {"_PeerExchange"}
 
 
 def entry_points():
@@ -109,7 +124,7 @@ def package_callers():
                 continue
             _, tree = _parse(os.path.join(dirpath, fn))
             for node in tree.body:
-                if isinstance(node, ast.ClassDef) and (node.name in END_TO_END or
+                if isinstance(node, ast.ClassDef) and (node.name in END_TO_END | MULTI_RANK or
                                                        any(getattr(bs, "id", None) in END_TO_END for bs in node.bases)):
                     continue
                 if isinstance(node, (ast.ClassDef, ast.FunctionDef)):
@@ -304,3 +319,76 @@ def test_names_resolve_through_imports_only():
     assert _test_module_reach(getter, wrappers, callers) == {"mg_conv_thin", "mg_maxpool_mask"}
     direct = ast.parse("def test_x(lib):\n    lib.load().mg_edge_weight(0)\n")
     assert _test_module_reach(direct, wrappers, callers) == {"mg_edge_weight"}
+
+
+# ============================================================================================== backward stages
+def backward_functions():
+    """The hand-written backward functions of the package -> their AST nodes: the module-level `*_bwd` functions of
+    networks/autograd.py, the `backward` of its autograd.Function classes ("Cls.backward") and every `backward_nhwc`
+    method under networks/ ("Cls.backward_nhwc")."""
+    net = os.path.join(PKG, "networks")
+    _, tree = _parse(os.path.join(net, "autograd.py"))
+    out = {}
+    for node in tree.body:
+        if isinstance(node, ast.FunctionDef) and node.name.endswith("_bwd"):
+            out[node.name] = node
+        elif isinstance(node, ast.ClassDef) and any(getattr(b, "attr", None) == "Function" for b in node.bases):
+            out.update({node.name + ".backward": m for m in node.body if isinstance(m, ast.FunctionDef) and m.name == "backward"})
+    for fn in sorted(os.listdir(net)):
+        if fn.endswith(".py"):
+            _, t = _parse(os.path.join(net, fn))
+            for node in t.body:
+                if isinstance(node, ast.ClassDef):
+                    out.update({node.name + ".backward_nhwc": m for m in node.body
+                                if isinstance(m, ast.FunctionDef) and m.name == "backward_nhwc"})
+    return out
+
+
+def backward_reach(tree, bwd):
+    """The backward functions a module's code reaches: a function it names, a method whose class and name it both names,
+    and, transitively, the backward functions their code names in turn."""
+    def named(q, names):
+        return all(part in names for part in q.split("."))
+    reached, todo = set(), [q for q in bwd if named(q, _code_names(tree))]
+    while todo:
+        q = todo.pop()
+        if q in reached:
+            continue
+        reached.add(q)
+        inner = _code_names(bwd[q])
+        todo.extend(r for r in bwd if r not in reached and named(r, inner))
+    return reached
+
+
+def test_backward_functions_are_found():
+    bwd = backward_functions()
+    assert {"block_bwd", "_spade_conv_bwd", "fc_bwd", "bg_bwd", "latent_bwd", "sn_conv_stack_bwd", "conv_encoder_bwd",
+            "_d_scale_bwd", "_DiscriminatorFn.backward", "ImageEncoder3.backward_nhwc", "ImageEncoder2.backward_nhwc",
+            "ImageEncoder.backward_nhwc"} <= set(bwd), sorted(bwd)
+
+
+def test_every_backward_function_has_a_stage_test():
+    bwd = backward_functions()
+    _, tree = _parse(os.path.join(TESTS, BACKWARD_STAGES_MODULE))
+    reached = backward_reach(tree, bwd)
+    assert set(NOT_IN_BACKWARD_STAGES) <= set(bwd), sorted(set(NOT_IN_BACKWARD_STAGES) - set(bwd))
+    missing = sorted(q for q in bwd if q not in reached and q not in NOT_IN_BACKWARD_STAGES)
+    assert not missing, ("backward functions %s does not reach (add a stage test, or list them in NOT_IN_BACKWARD_STAGES "
+                         "with a reason): %s" % (BACKWARD_STAGES_MODULE, missing))
+    stale = sorted(q for q in NOT_IN_BACKWARD_STAGES if q in reached)
+    assert not stale, "listed as left out but reached by %s: %s" % (BACKWARD_STAGES_MODULE, stale)
+
+
+def test_backward_reach_follows_calls_and_needs_the_class():
+    """A stage reached only through another backward function counts; a backward_nhwc counts only where its class is named
+    too; a backward function the module stops calling is missing."""
+    bwd = backward_functions()
+    tree = ast.parse("from michigan_b200.networks import autograd, ImageEncoder2\n\n"
+                     "def test_x(E, S):\n    autograd.block_bwd(None, None, S, None, None, None)\n"
+                     "    assert isinstance(E, ImageEncoder2)\n    E.backward_nhwc(None, S, None)\n")
+    reached = backward_reach(tree, bwd)
+    assert {"block_bwd", "_spade_conv_bwd", "ImageEncoder2.backward_nhwc", "sn_conv_stack_bwd"} <= reached
+    assert "ImageEncoder.backward_nhwc" not in reached and "bg_bwd" not in reached
+    _, full = _parse(os.path.join(TESTS, BACKWARD_STAGES_MODULE))
+    src = ast.unparse(full).replace("autograd.bg_bwd(", "autograd.block_bwd(")
+    assert "bg_bwd" not in backward_reach(ast.parse(src), bwd)
